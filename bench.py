@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- diffusion steps/sec of the PoseDiffusion sampling hot path on B200 (BASELINE.json metric).
+"""bench.py -- diffusion steps/sec of the PoseDiffusion sampling hot path on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload cfg3|cfg1|cfg2|cfg4|cfg5]
+                    [--dump-outputs DIR]
     (N > 1: launched by torchrun, one rank per GPU over NCCL)
 
 A bench "step" is one full p_sample_loop of the workload: T = 100 diffusion steps of one 20-frame sequence per GPU,
@@ -12,6 +13,9 @@ Output: ONE JSON line on rank 0 (see the contract in the task statement): value 
 e2e (host buffers through the C-ABI call, H2D/D2H and match packing inside the timed region), roofline of the
 dominant kernel (GGS/Sampson, HBM-bound, algorithmic 16 B per match-evaluation), cpu_baseline (the CPU oracle
 port on this box's host cores, bounded sample, extrapolated), clocks, gpu_launches.
+
+--dump-outputs DIR writes what the last timed step returned (DIR/pose.npy, or DIR/features.npy for --workload features) as
+float32; the inputs depend only on --seed, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -51,7 +55,7 @@ def read_peaks():
     if os.path.exists(path):
         with open(path) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback: H100 SXM data sheet, 3.35 TB/s HBM3 (not measured)"
 
 
 class ClockSampler:
@@ -97,9 +101,9 @@ class ClockSampler:
 
 
 # ----------------------------------------------------------------------------------------------------
-# CPU arm.  The reference is Python: its unmodified `models` / `util` packages are imported from /root/reference (build
-# container) or from baseline/_ref (installed by oracle/install_reference.py; what the GPU box has) behind the pytorch3d /
-# hydra shim of oracle/shims -> kind "reference".  If neither exists the oracle port (oracle/pose_oracle.py, the same operator
+# CPU arm.  The reference is Python: its unmodified `models` / `util` packages are imported from a reference checkout or
+# from oracle/_ref (installed by oracle/install_reference.py during build()) behind the pytorch3d / hydra shim of
+# oracle/shims -> kind "reference".  If neither exists the oracle port (oracle/pose_oracle.py, the same operator
 # sequence restated) is timed instead -> kind "port".  Bounded sample, extrapolated to the full loop.
 # ----------------------------------------------------------------------------------------------------
 def host_thread_candidates():
@@ -215,6 +219,15 @@ def cpu_features_run(n_images: int, seed: int, threads: int):
     return {"images_per_s": n_images / dt, "threads": threads, "sample": f"{n_images} frames of 224x224 at 3 scales in {dt:.2f} s"}
 
 
+def dump_outputs(out_dir, **arrays):
+    """Write each tensor as out_dir/<name>.npy in float32 (the outputs of the last timed step; at most a few MB here)."""
+    if not out_dir:
+        return
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
+
+
 def features_main(args):
     rank = int(os.environ.get("RANK", "0"))
     frames = 20 * args.seqs_per_gpu
@@ -287,7 +300,7 @@ def features_main(args):
         torch.distributed.destroy_process_group()
         return 0
     peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else None
-    bf16 = float(peaks["bf16_tflops"]) if peaks else 2250.0
+    bf16 = float(peaks["bf16_tflops"]) if peaks else 989.0
     flops_call = frames * VIT_TOKENS_PER_IMAGE * VIT_GEMM_FLOPS_PER_TOKEN
     achieved = flops_call * args.steps / (gemm_ms / 1000.0) / 1e12 if gemm_ms else None
     line = {
@@ -299,10 +312,10 @@ def features_main(args):
         "e2e": {"value": frames * world * args.steps / float(e2e_s.item()), "unit": "images/s", "h2d_bytes_per_step": int(img_host.numel() * 4),
                 "d2h_bytes_per_step": int(frames * 384 * 4), "note": "C-ABI pdb_extract_features_host from pinned host memory"},
         "gpu_launches": int(launches), "clocks": clocks.summary(),
-        "roofline": {"kernel": "tc_linear_kernel (tcgen05.mma kind::tf32 + TMA; all projections of the backbone)", "bound": "tensor",
+        "roofline": {"kernel": "tc_linear_kernel (wgmma tf32 + TMA; all projections of the backbone)", "bound": "tensor",
                      "achieved": achieved, "peak": bf16 / 2, "unit": "TFLOP/s", "frac": achieved / (bf16 / 2) if achieved else None, "traffic": None,
                      "peak_source": ("half of the measured dense bf16 rate (MEASURED_PEAKS.json bf16_tflops): TF32 runs at half the bf16 rate"
-                                     if peaks else "fallback: half of the nominal 2.25 PFLOP/s bf16 rate"),
+                                     if peaks else "fallback: half of the H100 SXM data-sheet dense bf16 rate, 989 TFLOP/s (not measured)"),
                      "algorithmic_flops_per_call": flops_call, "gemm_launches_per_call": gemm_n // max(1, args.steps),
                      "gemm_ms_per_call": gemm_ms / max(1, args.steps),
                      "note": "fp32 operands staged by TMA (4 B/element): the 128x128 tiles are bound by operand delivery from L2, not by the tensor pipe"},
@@ -311,6 +324,7 @@ def features_main(args):
         res = cpu_features_run(96, args.seed, min(os.cpu_count() or 1, 32))
         line["cpu_baseline"] = {"value": res["images_per_s"], "unit": "images/s", "cores": res["threads"], "kind": "port", "sample": res["sample"]}
     print(json.dumps(line))
+    dump_outputs(args.dump_outputs, features=z)
     if world > 1:
         torch.distributed.destroy_process_group()
     return 0
@@ -330,7 +344,9 @@ def main():
     ap.add_argument("--ggs-layout", default="paired", choices=["plain", "paired"],
                     help="HBM layout of the packed match stream (csrc/ggs_layout.cuh); 'paired' is the library default, see DESIGN.md 4.1")
     ap.add_argument("--denoiser-engine", default="auto", choices=["auto", "fp32", "tf32"],
-                    help="auto = exact-fp32 persistent kernel below 128 tokens per GPU, tcgen05/TMA tiles (TF32) at or above")
+                    help="auto = exact-fp32 persistent kernel below 128 tokens per GPU, wgmma/TMA tiles (TF32) at or above")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed to DIR/<name>.npy (float32; rank 0)")
     args = ap.parse_args()
     if args.seqs_per_gpu is None:
         args.seqs_per_gpu = 8 if args.workload == "cfg4" else 1
@@ -391,7 +407,7 @@ def main():
     z_dev, draws_dev = z_host.to(dev), draws_host.to(dev)
     problems = [ctx.pack_matches(m) for m in match_dicts] if per_pair else None
     m_total = problems[0].m_total if per_pair else 0
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     def one_loop():
         pose, _, _ = ctx.sample_loop(z_dev, draws_dev, problems, cfg if per_pair else None, start_step, want_trail=False, want_stats=False)
@@ -516,13 +532,14 @@ def main():
                      "and the iteration is latency-chain bound (run --workload cfg5 for the HBM-streaming case: 414 MB per inner iteration)")
                     if (args.workload == "cfg3" and B == 1) else
                     "algorithmic bytes = 16 B x matches x inner iterations, streamed every inner iteration through the TMA unit's bulk-async "
-                    "ring (from HBM at config 5: 414 MB per iteration; largely from L2 when the sequences' match sets fit its 126 MB)",
+                    "ring (from HBM at config 5: 414 MB per iteration; largely from L2 when the sequences' match sets fit its 50 MB)",
         }
     if not args.no_cpu_baseline and world == 1:  # reported baseline: rank 0 at N = 1 only
         res = cpu_reference_run(frames, per_pair, args.seed, args.cpu_budget)
         line["cpu_baseline"] = {"value": res["steps_per_s"], "unit": "diffusion steps/s", "cores": res["threads"], "kind": res["kind"],
                                 "sample": res["sample"], "wall_s_full_extrapolated": res["wall_s_full"]}
     print(json.dumps(line))
+    dump_outputs(args.dump_outputs, pose=full)
     if world > 1:
         torch.distributed.destroy_process_group()
     return 0

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""The reference's demo.py call pattern (pose_diffusion/demo.py:46-133) on the B200 path with synthetic inputs.
+"""The reference's demo.py call pattern (pose_diffusion/demo.py:46-133) on the native path with synthetic inputs.
 
 No checkpoint / DINO weights / hloc matches exist offline, so this script builds the model from the reference's config
 dict (cfgs/default.yaml), keeps the random initialisation, feeds random images through the native multi-scale DINO ViT-S/16

@@ -1,5 +1,5 @@
 /*
- * posediff_b200.h -- C ABI of the B200-native PoseDiffusion sampling hot path.
+ * posediff_b200.h -- C ABI of the H100-native PoseDiffusion sampling hot path.
  *
  * The reference (facebookresearch/PoseDiffusion) is pure Python + PyTorch ATen; it has NO C ABI,
  * plugin or FFI layer (SURVEY.md §8b).  This header therefore declares the entry points a
@@ -26,7 +26,7 @@
  * (NULL = legacy default stream).  All floating point data is IEEE fp32 unless stated; pose layout is the
  * reference's "absT_quaR_logFL" encoding [B, N, 9] = (T xyz, quaternion wxyz, log focal xy), row-major.
  * Every function returns PDB_OK (0) or a negative pdb_status; pdb_last_error() gives the message.
- * There is no CPU fallback: every compute entry point fails with PDB_ERR_CUDA if no sm_100 device exists.
+ * There is no CPU fallback: every compute entry point fails with PDB_ERR_CUDA if no sm_90 device exists.
  */
 #ifndef POSEDIFF_B200_H
 #define POSEDIFF_B200_H
@@ -42,7 +42,7 @@ extern "C" {
 typedef enum pdb_status {
   PDB_OK = 0,
   PDB_ERR_INVALID = -1,   /* bad argument (mirrors the reference's ValueError / NotImplementedError sites) */
-  PDB_ERR_CUDA = -2,      /* CUDA runtime failure, or no Blackwell device */
+  PDB_ERR_CUDA = -2,      /* CUDA runtime failure, or no Hopper (sm_90) device */
   PDB_ERR_STATE = -3,     /* e.g. weights not loaded */
   PDB_ERR_LIMIT = -4      /* size beyond a compiled limit (frames > PDB_MAX_FRAMES, ...) */
 } pdb_status;
@@ -96,21 +96,21 @@ int pdb_profile_read(pdb_context* ctx, double* ggs_ms, int64_t* ggs_launches, do
  * enable = 0 frees the buffer. */
 int pdb_debug_ggs_clocks(pdb_context* ctx, int32_t enable, int64_t* out, int32_t max_ctas);
 
-/* Swap-AB tcgen05 tiles (weights on the 128-row UMMA M side, 32 / 64 / 96 tokens on the N side) for GEMMs with at most 96 tokens
- * and O % 128 == 0; default off (measured slower than 128-token tiles without split-K).  Debug / measurement switch. */
+/* Swap-AB tensor-core tiles (weights on the 128-row M side, 32 / 64 / 96 tokens on the N side) for GEMMs with at most 96 tokens
+ * and O % 128 == 0; default off (without split-K only O/128 CTAs stream the weights).  Debug / measurement switch. */
 int pdb_debug_tc_swap(pdb_context* ctx, int32_t on);
 
 /* Stage hand-over inside the persistent fp32 denoiser kernel: 0 (default) = plain floats and a group barrier per stage; 1 = every
  * activation travels as a 64-bit {fp32, version tag} word and consumers poll the data itself, no barrier between the 43 stages of
- * a diffusion step.  Same arithmetic, bit-identical results; the flagged variant is ~3x slower (148 CTAs polling 80 KB tiles
- * saturate L2).  Debug / measurement switch (environment: PDB_DEN_FLAG). */
+ * a diffusion step.  Same arithmetic, bit-identical results; the flagged variant is slower (every CTA polling
+ * the 80 KB flagged tiles loads L2).  Debug / measurement switch (environment: PDB_DEN_FLAG). */
 int pdb_debug_denoiser_handover(pdb_context* ctx, int32_t flagged);
 
-/* Denoiser engine: 0 = auto (exact-fp32 persistent kernel below 128 tokens per GPU, tcgen05/TMA tensor-core tiles with TF32
+/* Denoiser engine: 0 = auto (exact-fp32 persistent kernel below 128 tokens per GPU, wgmma/TMA tensor-core tiles with TF32
  * products at or above), 1 = always fp32, 2 = always tensor cores. */
 int pdb_denoiser_engine(pdb_context* ctx, int32_t mode);
 
-/* Test entry of the tensor-core linear layer (tcgen05.mma kind::tf32 fed by TMA; csrc/tc_linear.cuh):
+/* Test entry of the tensor-core linear layer (wgmma tf32 fed by TMA; csrc/tc_linear.cuh):
  * Y[S,O] = relu?(X[S,K] @ W[O,K]^T + bias + residual); K % 32 == 0, O % 64 == 0, fp32 in / out, TF32 products. */
 int pdb_debug_tc_linear(pdb_context* ctx, const float* x_dev, const float* w_dev, const float* bias_dev,
                         const float* residual_dev, float* y_dev, int32_t S, int32_t O, int32_t K, int32_t relu,
@@ -223,7 +223,7 @@ int pdb_sample_loop_host_matches(pdb_context* ctx, const float* z_host, const fl
  * z = MultiScaleImageFeatureExtractor(image) (models/image_feature_extractor.py:27-87): the DINO ViT-S/16 backbone that the
  * reference pulls from torch.hub ("facebookresearch/dino:main", dino_vits16 -- third-party, restated in oracle/dino_vit.py),
  * applied to the ResNet-normalised image at each scale factor (bilinear resize, align_corners=False), class-token features
- * averaged over the scales (:74-83).  Projections run as tcgen05/TMA tiles with TF32 products (fp32 accumulate).
+ * averaged over the scales (:74-83).  Projections run as wgmma/TMA tiles with TF32 products (fp32 accumulate).
  *
  * `tensors[i]` (fp32, contiguous) in the hub checkpoint's state_dict order (`image_feature_extractor._net.*`): cls_token,
  * pos_embed[1,197,384], patch_embed.proj.{weight[384,3,16,16],bias}, then for block 0..11: norm1.{weight,bias},

@@ -1,14 +1,13 @@
-"""Install the UNMODIFIED reference hot-path packages into baseline/_ref (git-ignored; travels to the GPU box with gpurun).
+"""Install the UNMODIFIED reference hot-path packages into oracle/_ref (git-ignored build product).
 
-TEST / BENCH INFRASTRUCTURE.  The reference (`/root/reference`) is not a pip project (no setup.py / pyproject.toml), so the
-install the bench contract names (`pip install --no-index --no-build-isolation --target baseline/_ref /root/reference`)
-cannot work on the tree as it lies.  This script does what the contract allows instead: it copies `pose_diffusion/models` and
-`pose_diffusion/util` -- byte for byte -- to a scratch directory under /tmp, puts a three-line setup.py beside them there,
-and lets pip install that into baseline/_ref.  Nothing is written under /root/reference, nothing of the reference enters
-the tracked repository.  `oracle/ref_loader.py` imports the modules from baseline/_ref when /root/reference is absent (the
-GPU box), which lets `bench.py --impl reference` time the reference's OWN modules (`cpu_baseline.kind = "reference"`).
+TEST / BENCH INFRASTRUCTURE.  The reference checkout (POSEDIFF_REFERENCE_ROOT) is not a pip project (no setup.py /
+pyproject.toml), so this script copies `pose_diffusion/models` and `pose_diffusion/util` -- byte for byte -- to a temporary
+directory, puts a three-line setup.py beside them there, and lets pip install that into oracle/_ref.  Nothing is written into
+the reference checkout, nothing of the reference enters the tracked repository.  `oracle/ref_loader.py` imports the modules
+from oracle/_ref when the checkout itself is absent, which lets `bench.py --impl reference` time the reference's OWN modules
+(`cpu_baseline.kind = "reference"`).  Without a reference checkout nothing is installed and those legs time the oracle port.
 
-    python oracle/install_reference.py          # no-op when /root/reference is absent or baseline/_ref is up to date
+    python oracle/install_reference.py          # no-op without a reference checkout or when oracle/_ref is up to date
 """
 from __future__ import annotations
 
@@ -21,7 +20,7 @@ import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REFERENCE_ROOT = os.environ.get("POSEDIFF_REFERENCE_ROOT", "/root/reference")
-TARGET = os.path.join(ROOT, "baseline", "_ref")
+TARGET = os.path.join(ROOT, "oracle", "_ref")
 PACKAGES = ("models", "util")
 
 
@@ -56,13 +55,12 @@ def install(verbose: bool = True) -> str:
         if os.path.isdir(TARGET):
             shutil.rmtree(TARGET)
         os.makedirs(TARGET, exist_ok=True)
-        cmd = [sys.executable, "-m", "pip", "install", "--no-index", "--no-build-isolation", "--no-deps", "--find-links", "/opt/wheelhouse",
-               "--target", TARGET, tmp]
+        cmd = [sys.executable, "-m", "pip", "install", "--no-index", "--no-build-isolation", "--no-deps", "--target", TARGET, tmp]
         res = subprocess.run(cmd, capture_output=True, text=True)
         if res.returncode != 0:
             raise RuntimeError("pip install of the reference copy failed:\n" + res.stdout + res.stderr)
     if tree_digest(TARGET) != digest:
-        raise RuntimeError("baseline/_ref does not match the reference tree after the install")
+        raise RuntimeError("oracle/_ref does not match the reference tree after the install")
     with open(stamp, "w") as fh:
         fh.write(digest + "\n")
     if verbose:

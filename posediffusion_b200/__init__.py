@@ -1,4 +1,4 @@
-"""posediffusion_b200 -- B200-native (sm_100a) implementation of PoseDiffusion's sampling hot path.
+"""posediffusion_b200 -- H100-native (sm_90a) implementation of PoseDiffusion's sampling hot path.
 
 Public surface mirrors the reference's (`models.PoseDiffusionModel`, `models.GaussianDiffusion`,
 `models.Denoiser`, `util.geometry_guided_sampling.geometry_guided_sampling`,

@@ -1,7 +1,7 @@
 """ctypes binding of libposediff_b200.so (include/posediff_b200.h).
 
 PyTorch is used here only for device memory and streams.  There is NO fallback: if the library is
-missing, or no sm_100 GPU is present, every compute call raises.
+missing, or no sm_90 GPU is present, every compute call raises.
 """
 from __future__ import annotations
 
@@ -247,7 +247,7 @@ class Context:
     @classmethod
     def get(cls, device) -> "Context":
         if not torch.cuda.is_available():
-            raise NativeError("no CUDA device: posediffusion_b200 runs on B200 (sm_100a) only, there is no CPU fallback")
+            raise NativeError("no CUDA device: posediffusion_b200 runs on H100 (sm_90a) only, there is no CPU fallback")
         device = torch.device(device)
         index = device.index if device.index is not None else torch.cuda.current_device()
         if index not in cls._by_device:
@@ -286,7 +286,7 @@ class Context:
         self._ok(self.lib.pdb_debug_denoiser_handover(self.handle, int(flagged)), "pdb_debug_denoiser_handover")
 
     def set_tc_swap(self, on: bool):
-        """Swap-AB tcgen05 tiles for GEMMs with at most 96 tokens (default off; see profiles/r2_bench_tc_small.json)."""
+        """Swap-AB tensor-core tiles for GEMMs with at most 96 tokens (default off)."""
         self._ok(self.lib.pdb_debug_tc_swap(self.handle, int(on)), "pdb_debug_tc_swap")
 
     def set_ggs_layout(self, layout: str = "plain"):
@@ -296,7 +296,7 @@ class Context:
 
     def tc_linear(self, x: torch.Tensor, w: torch.Tensor, bias=None, residual=None, relu: bool = False,
                   in_place: bool = False) -> torch.Tensor:
-        """Y = relu?(x @ w^T + bias + residual) on the tcgen05 tensor cores (TF32 products, fp32 accumulate).
+        """Y = relu?(x @ w^T + bias + residual) on the tensor cores (wgmma, TF32 products, fp32 accumulate).
         in_place: Y is the residual buffer itself (the denoiser's residual-stream update; small problems then split K)."""
         S, K = x.shape
         O = w.shape[0]

@@ -1,4 +1,4 @@
-"""Build libposediff_b200.so in-tree with nvcc for sm_100a (no torch headers, CUDA runtime only).
+"""Build libposediff_b200.so in-tree with nvcc for sm_90a (no torch headers, CUDA runtime only).
 
     python -m posediffusion_b200.build [--force]
 
@@ -18,7 +18,7 @@ CSRC = os.path.join(PKG, "csrc")
 OBJ = os.path.join(ROOT, "build", "obj")
 LIB = os.path.join(PKG, "libposediff_b200.so")
 SOURCES = ["api_core.cu", "api_sampler.cu", "api_tc.cu", "api_vit.cu", "api_post.cu"]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xptxas", "-v", f"-I{os.path.join(ROOT, 'include')}", f"-I{CSRC}"]
 
 

@@ -84,8 +84,8 @@ int pdb_create(pdb_context** out, int device_ordinal) {
     g_create_error = cudaGetErrorString(err);
     return PDB_ERR_CUDA;
   }
-  if (prop.major != 10) {
-    g_create_error = "posediff_b200 is built for sm_100a only; device is sm_" + std::to_string(prop.major) + std::to_string(prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    g_create_error = "posediff_b200 is built for sm_90a only; device is sm_" + std::to_string(prop.major) + std::to_string(prop.minor);
     return PDB_ERR_CUDA;
   }
   if ((err = cudaSetDevice(device_ordinal)) != cudaSuccess) {

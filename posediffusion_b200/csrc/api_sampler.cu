@@ -138,7 +138,7 @@ int enqueue_denoiser(Context* ctx, DenoiserRun run, cudaStream_t st) {
   if (run.t_hi >= kT || run.t_lo < 0 || run.t_hi < run.t_lo) return ctx->fail(PDB_ERR_INVALID, "bad timestep range");
   const int S = run.batch * run.frames;
   run.tokens = S;
-  // engine: exact-fp32 persistent kernel below kTcMinTokens tokens (latency bound), tcgen05/TMA tiles (TF32 products) at or
+  // engine: exact-fp32 persistent kernel below kTcMinTokens tokens (latency bound), wgmma/TMA tiles (TF32 products) at or
   // above it (throughput bound).  ctx->denoiser_engine: 0 auto, 1 force fp32, 2 force tensor cores.
   const bool use_tc = ctx->denoiser_engine == 2 || (ctx->denoiser_engine == 0 && S >= kTcMinTokens);
   if (use_tc) return enqueue_denoiser_tc(ctx, run, st);

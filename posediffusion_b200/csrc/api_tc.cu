@@ -1,4 +1,4 @@
-// Tensor-core (tcgen05 + TMA) linear layer: host side (tensor maps, launch) and a test entry point.
+// Tensor-core (wgmma + TMA) linear layer: host side (tensor maps, launch) and a test entry point.
 #include <cuda.h>
 #include <cudaTypedefs.h>
 
@@ -61,6 +61,15 @@ int make_map(Context* ctx, CUtensorMap* map, const float* ptr, int rows, int K, 
 
 namespace pdb {
 
+// Persistent grid: as many CTAs as are resident on the GPU at once (shared memory and registers decide).  Kernel and
+// shared-memory size are fixed per instantiation, so the answer is cached by the caller.
+template <typename Kernel>
+static int resident_ctas(const Context* ctx, Kernel kernel, size_t smem) {
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kTcThreads, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+  return per_sm * ctx->sm_count;
+}
+
 // Y = epilogue(X[S,K] @ W[O,K]^T) on the tensor cores.  K % 32 == 0, O % 64 == 0, all pointers 16-byte aligned.
 template <int BN, int ST>
 static int launch_tc_linear(Context* ctx, const float* X, const float* W, const TcEpilogue& E, bool& attr, cudaStream_t st) {
@@ -68,13 +77,14 @@ static int launch_tc_linear(Context* ctx, const float* X, const float* W, const 
   if (int rc = make_map(ctx, &mx, X, E.S, E.K, kTcBM)) return rc;
   if (int rc = make_map(ctx, &mw, W, E.O, E.K, BN)) return rc;
   const size_t smem = tc_smem_bytes(BN, ST);
+  static int resident = 0;
   if (!attr) {
     PDB_CUDA(ctx, cudaFuncSetAttribute(tc_linear_kernel<BN, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    resident = resident_ctas(ctx, tc_linear_kernel<BN, ST>, smem);
     attr = true;
   }
   const int tiles = (E.O / BN) * ((E.S + kTcBM - 1) / kTcBM) * (E.splits > 1 ? E.splits : 1);
-  // two CTAs per SM where the ring allows it (shared memory and 2 x 2BN <= 512 TMEM columns); the 8-deep ring fills an SM
-  const int grid = std::min(tiles, (2 * smem <= ctx->smem_optin ? 2 : 1) * ctx->sm_count);
+  const int grid = std::min(tiles, resident);
   {
     ScopedTimer timer(ctx, st, 1);
     PDB_CUDA(ctx, launch_chained(tc_linear_kernel<BN, ST>, dim3(grid), dim3(kTcThreads), smem, st, E.pdl != 0, mx, mw, E));
@@ -91,12 +101,14 @@ static int launch_tc_linear_swap(Context* ctx, const float* X, const float* W, c
   if (int rc = make_map(ctx, &mx, X, E.S, E.K, NT)) return rc;
   if (int rc = make_map(ctx, &mw, W, E.O, E.K, kTcBM)) return rc;
   const size_t smem = tc_smem_bytes(NT, kTcStages);
+  static int resident = 0;
   if (!attr) {
     PDB_CUDA(ctx, (cudaFuncSetAttribute(tc_linear_kernel<NT, kTcStages, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)));
+    resident = resident_ctas(ctx, tc_linear_kernel<NT, kTcStages, true>, smem);
     attr = true;
   }
   const int tiles = (E.O / kTcBM) * ((E.S + NT - 1) / NT);
-  const int grid = std::min(tiles, 2 * ctx->sm_count);
+  const int grid = std::min(tiles, resident);
   {
     ScopedTimer timer(ctx, st, 1);
     tc_linear_kernel<NT, kTcStages, true><<<grid, kTcThreads, smem, st>>>(mx, mw, E);
@@ -107,15 +119,14 @@ static int launch_tc_linear_swap(Context* ctx, const float* X, const float* W, c
 }
 
 // Swap-AB tiles are taken for at most 96 tokens when enabled (pdb_debug_tc_swap / PDB_TC_SWAP=1).  Default off: without split-K
-// only O/128 CTAs stream the weights and the tile is bound by one SM's L2 bandwidth (profiles/r2_bench_tc_small.json: slower
-// than padding the tokens to a 128-row tile except at 5 tokens).
+// only O/128 CTAs stream the weights and the tile is bound by one SM's L2 bandwidth.
 static bool tc_linear_swapped(const Context* ctx, int S, int O) {
   static const bool env_on = [] { const char* v = getenv("PDB_TC_SWAP"); return v && v[0] == '1'; }();
   return S <= 96 && O % kTcBM == 0 && (env_on || ctx->tc_swap);
 }
 
 // Y = epilogue(X[S,K] @ W[O,K]^T) on the tensor cores.  K % 32 == 0, O % 64 == 0, all pointers 16-byte aligned.
-// 128-feature tiles (UMMA 128x128x8) when they still fill the machine, 64-feature tiles for the small-S denoiser shapes,
+// 128-feature tiles (two wgmma 64x128x8 per K-step) when they still fill the machine, 64-feature tiles for the small-S denoiser shapes,
 // swap-AB tiles (weights on the M side) for at most 96 tokens when enabled (pdb_debug_tc_swap / PDB_TC_SWAP=1).
 int enqueue_tc_linear(Context* ctx, const float* X, const float* W, TcEpilogue E, cudaStream_t st) {
   if (E.K % kTcBK || E.O % 64 || E.S < 1) return ctx->fail(PDB_ERR_INVALID, "tc_linear shape (S=%d, O=%d, K=%d)", E.S, E.O, E.K);
@@ -126,14 +137,13 @@ int enqueue_tc_linear(Context* ctx, const float* X, const float* W, TcEpilogue E
     if (E.S <= 64) return launch_tc_linear_swap<64>(ctx, X, W, E, ctx->attr_tc_swap[1], st);
     return launch_tc_linear_swap<96>(ctx, X, W, E, ctx->attr_tc_swap[2], st);
   }
-  E.vec8 = (reinterpret_cast<uintptr_t>(E.Y) % 32 == 0) && (E.ldy % 8 == 0) &&
-           (!E.residual || (reinterpret_cast<uintptr_t>(E.residual) % 32 == 0 && E.ldr % 8 == 0));
   const long long wide_tiles = (long long)(E.O / 128) * ((E.S + kTcBM - 1) / kTcBM);
-  if (E.O % 128 == 0 && wide_tiles >= ctx->sm_count) {  // (measured: relaxing this to 85 % of the SMs is slower, 1.79 vs 1.67 ms per 20 frames)
-    // 3 x 32 KB ring: two CTAs per SM, the epilogue of one under the main loop of the other (measured 1.16-1.26x over 4 x 32 KB)
+  if (E.O % 128 == 0 && wide_tiles >= ctx->sm_count) {
+    // one CTA per SM (64 accumulator registers per consumer thread): a 6 x 32 KB ring lets the producer run half a K = 384
+    // tile ahead while the consumers are in the epilogue
     E.splits = 1;
     E.stats = 0;
-    return launch_tc_linear<128, 3>(ctx, X, W, E, ctx->attr_tc128, st);
+    return launch_tc_linear<128, 6>(ctx, X, W, E, ctx->attr_tc128, st);
   }
   if (E.allow_small && tc_linear_small(ctx, E.S, E.O)) {
     // Fewer 64-feature tiles than SMs (the denoiser at a few hundred tokens): a CTA's k-loop is a serial chain of TMA round
@@ -142,7 +152,7 @@ int enqueue_tc_linear(Context* ctx, const float* X, const float* W, TcEpilogue E
     // LayerNorm statistics come out of the X tiles inside the kernel (E.stats, requested by the caller).
     const int tiles = (E.O / 64) * ((E.S + kTcBM - 1) / kTcBM), num_kb = E.K / kTcBK;
     E.splits = 1;
-    const bool in_place = E.residual == E.Y && E.ldr == E.ldy && !E.relu && !E.gelu && !E.colsum && E.vec8;
+    const bool in_place = E.residual == E.Y && E.ldr == E.ldy && !E.relu && !E.gelu && !E.colsum;
     if (in_place)
       for (int s : {8, 4, 2})
         if (num_kb % s == 0 && num_kb / s >= 2 && tiles * s <= ctx->sm_count) {
@@ -187,7 +197,7 @@ extern "C" int pdb_debug_tc_linear(pdb_context* c, const float* x_dev, const flo
 }
 
 // ================================================================================================
-// Tensor-core denoiser engine (S >= 128 tokens per GPU): one kernel per stage, projections on tcgen05/TMA tiles.
+// Tensor-core denoiser engine (S >= 128 tokens per GPU): one kernel per stage, projections on wgmma/TMA tiles.
 // Same maths as denoiser_kernel (csrc/denoiser.cuh); LayerNorm is folded into the QKV / FF1 weights at load time and
 // applied in the GEMM epilogue from per-row statistics.  TF32 products, fp32 accumulate / residual stream.
 // ================================================================================================
@@ -316,8 +326,8 @@ int enqueue_denoiser_tc(Context* ctx, DenoiserRun run, cudaStream_t st) {
   // captured once per buffer set, replayed per step ----
   const bool stats_qkv = tc_linear_small(ctx, S, 3 * kDM), stats_ff1 = tc_linear_small(ctx, S, kFF);
   auto enqueue_step = [&](cudaStream_t s) -> int {
-    // the kernels of a step form one programmatic chain (the first one has no predecessor in the capture).  Measured on the
-    // denoiser per 100 steps: 160 tokens 34.7 -> 33.1 ms, 640 tokens 41.5 -> 43.3 ms, 2560 tokens 69.8 -> 70.1 ms: small steps only
+    // the kernels of a step form one programmatic chain (the first one has no predecessor in the capture); only small steps
+    // gain from overlapping a kernel's prologue with its predecessor's tail
     pdl = ctx->tc_pdl && S <= 320;
     PDB_CUDA(ctx, launch_chained(embed_kernel, dim3((S * kPoseEmbPad + 255) / 256), dim3(256), 0, s, false, (const float*)run.x, emb, S));
     if (int rc = lin(emb, T.wx, kDM, kPoseEmbPad, T.tproj, tstate, run.zproj, kDM, nullptr, run.h, 0, s)) return rc;

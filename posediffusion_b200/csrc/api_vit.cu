@@ -2,8 +2,8 @@
 // (torch.hub facebookresearch/dino:main `vit_small(patch_size=16)`, restated in oracle/dino_vit.py) applied to the ResNet-normalised
 // image at every scale factor, class-token features averaged over the scales.
 //
-// B200 layout: the tokens of ALL scales and images form one [S_total, 384] activation matrix (scale-major, then image, then
-// token; 197 + 50 + 17 tokens per 224^2 image at the default scales), so that every projection of a block is ONE tcgen05/TMA
+// Layout: the tokens of ALL scales and images form one [S_total, 384] activation matrix (scale-major, then image, then
+// token; 197 + 50 + 17 tokens per 224^2 image at the default scales), so that every projection of a block is ONE wgmma/TMA
 // GEMM (csrc/tc_linear.cuh, TF32 products, fp32 accumulate) over all of them:
 //   patchify (normalise + bilinear resize + im2col, fused) -> GEMM [S,768]x[768,384] -> + class token / position table
 //   12 x { row stats -> GEMM qkv (LayerNorm folded into the weights, applied in the epilogue) -> attention (shared memory,
@@ -205,7 +205,7 @@ __global__ void vit_row_stats_kernel(const float* __restrict__ X, float* __restr
 }
 
 // Multi-head self-attention of one (image, scale) sequence of L <= 256 tokens, head width 64, on the warp-level tensor-core path
-// (mma.sync m16n8k8 TF32, fp32 accumulate): the problem is 197 x 197 x 64 per head -- far below a 128-row tcgen05 tile pipeline's
+// (mma.sync m16n8k8 TF32, fp32 accumulate): the problem is 197 x 197 x 64 per head -- far below a 128-row wgmma tile pipeline's
 // break-even -- so each warp owns 16 query rows end to end and the logits never leave registers:
 //   S = (Q / 8) K^T   : A = Q fragments (registers, from global), B = K rows from shared memory (row stride 68 words: the 32
 //                       lanes of a B-fragment load hit 32 distinct banks), in blocks of 8 key tiles (64 keys);

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the posediff_b200 kernels (sm_100a only).
+// Shared device/host helpers for the posediff_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -160,7 +160,7 @@ __device__ __forceinline__ unsigned long long ld_ll(const unsigned long long* p)
   return w;
 }
 // Programmatic dependent launch (kernels chained inside the tensor-core engine's step graph): `pdl_trigger` lets the next kernel
-// of the chain start its prologue (barrier init, TMEM allocation, descriptor prefetch) while this one is still running;
+// of the chain start its prologue (barrier init, descriptor prefetch) while this one is still running;
 // `pdl_wait` blocks until the previous kernel has completed and its writes are visible.  Both are no-ops in a kernel that was
 // not launched with the programmatic-serialization attribute.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -178,7 +178,7 @@ __device__ __forceinline__ void ll_backoff() {}
 // One-hop all-reduce accumulators: {fp32 sum, fp32 arrivals} in one 8-byte word.  ONE vector reduction adds {v, 1.0} to the
 // pair (red.v2.f32, sm_90+); a reader that sees the expected number of arrivals has the complete sum.  PTX only promises
 // per-element atomicity of a vector reduction; on this hardware both elements of the 8-byte-aligned pair are applied by the
-// L2 reduction unit in one pass (tools/xchg_probe.cu mode 8 watches for torn pairs: none in 4e8 polls, see profiles/).
+// L2 reduction unit in one pass (tools/xchg_probe.cu mode 8 watches for torn pairs).
 __device__ __forceinline__ void red_pair_add(float* p, float v) {
   asm volatile("red.relaxed.gpu.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(v), "f"(1.0f) : "memory");
 }

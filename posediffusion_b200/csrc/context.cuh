@@ -29,8 +29,8 @@ struct Context {
   void* den_ws = nullptr;
   size_t den_ws_bytes = 0;
   // stage hand-over of the persistent denoiser kernel: 0 = group barriers (default), 1 = flag-carrying activation words, no
-  // barriers (pdb_debug_denoiser_handover / PDB_DEN_FLAG; parity-identical but 3x slower: 148 CTAs polling an 80 KB tile saturate
-  // L2, profiles/r2_negative_den_flagged_*.txt)
+  // barriers (pdb_debug_denoiser_handover / PDB_DEN_FLAG; parity-identical but slower: every CTA polling an 80 KB tile
+  // loads L2)
   int den_flag = 0;
   void* den_flag_ws = nullptr;
   size_t den_flag_ws_bytes = 0;
@@ -49,7 +49,7 @@ struct Context {
   size_t attr_ggs[8] = {0, 0, 0, 0, 0, 0, 0, 0}, attr_den[16] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0}, attr_att = 0;
   bool attr_tc = false, attr_tc128 = false, attr_tc_deep = false;
   bool tc_pdl = true;  // programmatic dependent launch between the kernels of the tensor-core engine's step graph (PDB_TC_PDL=0: off)
-  bool tc_swap = false;     // swap-AB tcgen05 tiles for <= 96 tokens (pdb_debug_tc_swap); default off, see profiles/r2_bench_tc_small.json
+  bool tc_swap = false;     // swap-AB tensor-core tiles for <= 96 tokens (pdb_debug_tc_swap); default off
   bool attr_tc_swap[3] = {false, false, false};  // swap-AB instantiations (32 / 64 / 96 tokens on the N side)
   // image feature extractor (csrc/api_vit.cu)
   VitWeights* vit = nullptr;
@@ -57,7 +57,7 @@ struct Context {
   size_t vit_ws_bytes = 0;
   size_t attr_vit_att[4] = {0, 0, 0, 0};
   int ggs_layout = 1;       // stream layout of match sets packed on this context (ggs_layout.cuh): 0 plain, 1 paired (default)
-  int denoiser_engine = 0;  // 0 auto, 1 fp32 persistent kernel, 2 tcgen05/TMA tiles (TF32)
+  int denoiser_engine = 0;  // 0 auto, 1 fp32 persistent kernel, 2 wgmma/TMA tiles (TF32)
   // optional per-kernel timing (bench.py roofline): event pairs per launch, kind 0 = GGS, 1 = denoiser
   bool profiling = false;
   struct Timed { cudaEvent_t a, b; int kind; };

@@ -13,8 +13,7 @@
 // latency / weight-bandwidth bound (SURVEY.md §8d).
 //
 // Stage hand-over, two instantiations of the same kernel (kFlag = false is the product default; kFlag = true is bit-identical
-// in its results and measured 3x slower at 148 CTAs -- every CTA polling the 80 KB flagged tile saturates L2, see DESIGN.md
-// §4.4 and tools/stage_probe.cu -- and stays as a tested alternative behind pdb_debug_denoiser_handover):
+// in its results and slower -- every CTA polls the 80 KB flagged tile through L2, see tools/stage_probe.cu -- and stays as a tested alternative behind pdb_debug_denoiser_handover):
 //   kFlag = false  activations are plain floats in global memory; a group barrier (block barrier, release reduction,
 //                  acquire poll) separates consecutive stages.
 //   kFlag = true   every activation is published as ONE 64-bit word {fp32 value, 32-bit version tag} with a relaxed store

@@ -70,7 +70,7 @@ struct GgsParams {
   int xch_group;        // CTAs per exchange group; >= ctas_per_problem: one-level exchange (every CTA reads every slot)
   int xch_mode;         // 0: flag-carrying words through slots (xch1 / xch2); 1: one hop through vector reductions (acc)
 };
-constexpr int kAccStride = 32;  // floats between two accumulators: one 128-byte line each (148 CTAs adding into neighbouring
+constexpr int kAccStride = 32;  // floats between two accumulators: one 128-byte line each (one CTA per SM adding into neighbouring
                                 // sectors serialise on a few L2 slices: 3.4 us per all-reduce at 32 B, 2.2 us at 128 B, tools/xchg_probe.cu)
 
 __host__ __device__ inline int ggs_xch_words(int frames) { return frames * 7 + kAccTail; }
@@ -86,39 +86,50 @@ __host__ __device__ inline size_t ggs_smem_fixed_bytes(int frames) {
   return (bytes + 127) / 128 * 128;
 }
 
-// Two matches per instruction: Blackwell's packed fp32x2 pipe (FFMA2 / FMUL2 / FADD2) halves the issue slots of the
-// arithmetic that dominates stage 1.  Same formulas as `sampson_match` (geom.cuh) for two in-bounds rows A and B of the
-// same pair; acc2[k] holds separate partial sums for the two rows (merged at the segment end).
+// Element-wise float2 arithmetic, one match per component.  Correctly rounded FMA / multiply / add: __fmul_rn and __fadd_rn are
+// never contracted into an FMA, so every component is rounded exactly as the formula is written.
+#ifdef PDB_EMU
+inline float2 fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+inline float2 mul2(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
+inline float2 add2(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
+#else
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+#endif
+// Two matches per call: two independent dependency chains interleaved, which keeps the FMA pipe busy in stage 1.  Same
+// formulas as `sampson_match` (geom.cuh) for two in-bounds rows A and B of the same pair; acc2[k] holds separate partial
+// sums for the two rows (merged at the segment end).
 __device__ __forceinline__ void sampson_match2_core(const float2 u1, const float2 v1, const float2 u2, const float2 v2,
                                                     const float* __restrict__ F, float smax, float2* __restrict__ acc2) {
-  float2 F2[9];  // (F'[k], F'[k]): the packed pipe reads a scalar register as a broadcast pair (R.F32 operand form)
+  float2 F2[9];  // (F'[k], F'[k])
 #pragma unroll
   for (int k = 0; k < 9; ++k) F2[k] = make_float2(F[k], F[k]);
-  const float2 l0 = __ffma2_rn(u1, F2[0], __ffma2_rn(v1, F2[3], F2[6]));
-  const float2 l1 = __ffma2_rn(u1, F2[1], __ffma2_rn(v1, F2[4], F2[7]));
-  const float2 l2 = __ffma2_rn(u1, F2[2], __ffma2_rn(v1, F2[5], F2[8]));
-  const float2 r0 = __ffma2_rn(F2[0], u2, __ffma2_rn(F2[1], v2, F2[2]));
-  const float2 r1 = __ffma2_rn(F2[3], u2, __ffma2_rn(F2[4], v2, F2[5]));
-  const float2 top = __ffma2_rn(l0, u2, __ffma2_rn(l1, v2, l2));
-  const float2 bottom = __ffma2_rn(l0, l0, __ffma2_rn(l1, l1, __ffma2_rn(r0, r0, __fmul2_rn(r1, r1))));
-  const float2 t = __fmul2_rn(top, make_float2(fast_rcp(bottom.x), fast_rcp(bottom.y)));
-  const float2 err = __fmul2_rn(top, t);
+  const float2 l0 = fma2(u1, F2[0], fma2(v1, F2[3], F2[6]));
+  const float2 l1 = fma2(u1, F2[1], fma2(v1, F2[4], F2[7]));
+  const float2 l2 = fma2(u1, F2[2], fma2(v1, F2[5], F2[8]));
+  const float2 r0 = fma2(F2[0], u2, fma2(F2[1], v2, F2[2]));
+  const float2 r1 = fma2(F2[3], u2, fma2(F2[4], v2, F2[5]));
+  const float2 top = fma2(l0, u2, fma2(l1, v2, l2));
+  const float2 bottom = fma2(l0, l0, fma2(l1, l1, fma2(r0, r0, mul2(r1, r1))));
+  const float2 t = mul2(top, make_float2(fast_rcp(bottom.x), fast_rcp(bottom.y)));
+  const float2 err = mul2(top, t);
   const float2 wgt = make_float2(err.x < smax ? 1.f : 0.f, err.y < smax ? 1.f : 0.f);
-  const float2 a = __fmul2_rn(wgt, __fadd2_rn(t, t));
-  const float2 nb = __fmul2_rn(a, make_float2(-t.x, -t.y));
-  acc2[9] = __fadd2_rn(acc2[9], make_float2(err.x > smax ? smax : err.x, err.y > smax ? smax : err.y));
-  acc2[11] = __fadd2_rn(acc2[11], wgt);
-  const float2 w0 = __ffma2_rn(a, u2, __fmul2_rn(nb, l0)), w1 = __ffma2_rn(a, v2, __fmul2_rn(nb, l1));
-  const float2 c0 = __fmul2_rn(nb, r0), c1 = __fmul2_rn(nb, r1);
-  acc2[0] = __ffma2_rn(c0, u2, __ffma2_rn(u1, w0, acc2[0]));
-  acc2[1] = __ffma2_rn(c0, v2, __ffma2_rn(u1, w1, acc2[1]));
-  acc2[2] = __fadd2_rn(__ffma2_rn(u1, a, acc2[2]), c0);
-  acc2[3] = __ffma2_rn(c1, u2, __ffma2_rn(v1, w0, acc2[3]));
-  acc2[4] = __ffma2_rn(c1, v2, __ffma2_rn(v1, w1, acc2[4]));
-  acc2[5] = __fadd2_rn(__ffma2_rn(v1, a, acc2[5]), c1);
-  acc2[6] = __fadd2_rn(acc2[6], w0);
-  acc2[7] = __fadd2_rn(acc2[7], w1);
-  acc2[8] = __fadd2_rn(acc2[8], a);
+  const float2 a = mul2(wgt, add2(t, t));
+  const float2 nb = mul2(a, make_float2(-t.x, -t.y));
+  acc2[9] = add2(acc2[9], make_float2(err.x > smax ? smax : err.x, err.y > smax ? smax : err.y));
+  acc2[11] = add2(acc2[11], wgt);
+  const float2 w0 = fma2(a, u2, mul2(nb, l0)), w1 = fma2(a, v2, mul2(nb, l1));
+  const float2 c0 = mul2(nb, r0), c1 = mul2(nb, r1);
+  acc2[0] = fma2(c0, u2, fma2(u1, w0, acc2[0]));
+  acc2[1] = fma2(c0, v2, fma2(u1, w1, acc2[1]));
+  acc2[2] = add2(fma2(u1, a, acc2[2]), c0);
+  acc2[3] = fma2(c1, u2, fma2(v1, w0, acc2[3]));
+  acc2[4] = fma2(c1, v2, fma2(v1, w1, acc2[4]));
+  acc2[5] = add2(fma2(v1, a, acc2[5]), c1);
+  acc2[6] = add2(acc2[6], w0);
+  acc2[7] = add2(acc2[7], w1);
+  acc2[8] = add2(acc2[8], a);
 }
 // plain layout: the rows of two rounds, one float4 (u1,v1,u2,v2) each -> the compiler re-pairs the components (MOVs)
 __device__ __forceinline__ void sampson_match2(const float4 A, const float4 B, const float* __restrict__ F, float smax,
@@ -222,8 +233,7 @@ __device__ __noinline__ void ggs_exchange(unsigned long long* xch1, unsigned lon
 // `resident_rounds` > 0: the CTA's whole slice of matches (<= resident_rounds rounds) is staged in shared memory
 // once per launch and every inner iteration streams it from there (no L2/HBM traffic inside the loop).
 // kProbe: the stage timing probe (tools/ggs_stage_probe.py) is a separate instantiation, so that the production kernels carry no
-// clock reads: the code one iteration executes (1 871 instructions = 255 lines of 128 B with the probe) sits right at the 32 KB
-// capacity of the L1.5 instruction cache (hit rate 85 %, profiles/r2_ggs_cfg3_ncu_raw.csv).
+// clock reads: the code one iteration executes is close to the capacity of the instruction cache.
 template <bool kEval, bool kPaired = false, bool kProbe = false>
 __device__ __forceinline__ void ggs_body(const GgsProblem& pr, const GgsParams& P) {
 #ifdef PDB_EMU  // tests/host/cuda_emu.h (CPU emulation of this kernel, test harness only): dynamic shared memory of this CTA

@@ -8,9 +8,8 @@
 //            A = row 64 U + l and B = row 64 U + 32 + l of the plain order, stored component-interleaved:
 //                pts[64 U + l]      = (u1_A, u1_B, v1_A, v1_B)
 //                pts[64 U + 32 + l] = (u2_A, u2_B, v2_A, v2_B)
-//            so that the two 128-bit loads of a lane land as the aligned register pairs the packed fp32x2 pipe
-//            (FFMA2 / FMUL2 / FADD2) takes as operands.  With the plain layout the compiler has to re-pair the
-//            components of two float4 with ~45 MOVs per two matches (about as many issue slots as the arithmetic).
+//            so that the two 128-bit loads of a lane hold the two matches' operands side by side (sampson_match2_unit
+//            in ggs.cuh); with the plain layout the compiler re-pairs the components of two float4 with extra MOVs.
 //            Every segment starts at an even round and all partition boundaries are even, so a unit never straddles
 //            two segments, two warps or two CTAs.
 #pragma once

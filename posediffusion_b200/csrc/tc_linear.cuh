@@ -1,19 +1,19 @@
-// Tensor-core linear layer for the batched denoiser (S = B*N >= 128 tokens per GPU, BASELINE config 4):
+// Tensor-core linear layer for the batched denoiser (S = B*N >= 128 tokens per GPU, BASELINE config 4) and the ViT backbone:
 //   Y[S, O] = epilogue( X[S, K] @ W[O, K]^T )
-// as tcgen05 (5th-gen tensor core) tiles fed by TMA, written directly in PTX for sm_100a:
-//   * TMA (`cp.async.bulk.tensor.2d`) stages 128-token x 32-float (128 B, SWIZZLE_128B) boxes of X and BN-feature boxes of
-//     W into a 4-deep shared-memory ring, completion counted on mbarriers;
-//   * one elected thread issues `tcgen05.mma.cta_group::1.kind::tf32` (fp32 operands read as TF32, fp32 accumulate) with
-//     shared-memory descriptors, 4 K-steps of 8 per stage; the 128 x BN fp32 accumulator lives in TMEM;
-//   * the kernel is persistent over output tiles with a double-buffered TMEM accumulator (epilogue of tile i under the main loop of i+1);
-//   * `tcgen05.commit` releases ring slots / signals the epilogue; 4 epilogue warps read TMEM with `tcgen05.ld`
-//     (32 lanes x 32 columns per instruction) and apply bias / folded LayerNorm / residual / ReLU on the way to HBM.
-// Warp roles: 0 = TMA producer, 1 = TMEM allocator + MMA issuer, 2..5 = epilogue (one TMEM lane quarter each).
+// as Hopper warpgroup MMA tiles fed by TMA, written directly in PTX for sm_90a:
+//   * TMA (`cp.async.bulk.tensor.2d`) stages 128-row x 32-float (128 B, SWIZZLE_128B) boxes of the M-side operand and
+//     BN-row boxes of the N-side operand into a shared-memory ring, completion counted on mbarriers;
+//   * two consumer warpgroups each issue `wgmma.mma_async.m64nBNk8.f32.tf32.tf32` (fp32 operands read as TF32, fp32
+//     accumulate) on 64 of the tile's 128 M-side rows, both operands read from shared memory through descriptors, 4 K-steps of
+//     8 per stage; the 64 x BN fp32 accumulator of a warpgroup lives in its registers (BN / 2 per thread);
+//   * the kernel is persistent over output tiles; one wgmma group stays in flight while the previous stage is released, and
+//     the producer keeps filling the ring for the next tile while the consumers run the epilogue (bias / folded LayerNorm /
+//     residual / ReLU / GELU) from registers straight to global memory.
+// Warp roles: warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = MMA + epilogue (M-side rows 0-63 and 64-127).
 //
-// Swap-AB instantiation (kSwap, few tokens: S <= 96): the WEIGHTS take the 128-row UMMA M side (A = 128 features x 32 k) and
+// Swap-AB instantiation (kSwap, few tokens: S <= 96): the WEIGHTS take the 128-row M side (A = 128 features x 32 k) and
 // the tokens the N side (B = BN tokens x 32 k, BN = 32 / 64 / 96, rows beyond S zero-filled by TMA), i.e. the tile computes
-// Y^T[128 features, BN tokens].  No tensor-core work is spent on padding tokens up to 128 rows; an accumulator row (TMEM
-// lane) is a feature, so an epilogue warp stores 32 consecutive features of one token per instruction (128 contiguous bytes).
+// Y^T[128 features, BN tokens].  No tensor-core work is spent on padding tokens up to 128 rows.
 #pragma once
 #include <cuda.h>
 
@@ -21,10 +21,11 @@
 
 namespace pdb {
 
-constexpr int kTcThreads = 192;
-constexpr int kTcStages = 4;  // default ring depth (64-feature tiles); the 128-feature variant may run 3 deep so that two CTAs share an SM
-constexpr int kTcBM = 128;  // tokens per tile  (UMMA M)
-constexpr int kTcBK = 32;   // floats per stage (128 bytes = one swizzle atom), 4 UMMA K-steps of 8
+constexpr int kTcThreads = 384;
+constexpr int kTcStages = 4;  // default ring depth (64-feature tiles: two CTAs share an SM)
+constexpr int kTcBM = 128;  // M-side rows per tile (two warpgroups x wgmma M = 64)
+constexpr int kTcBK = 32;   // floats per stage (128 bytes = one swizzle atom), 4 wgmma K-steps of 8
+constexpr int kTcConsumerWarps = 8;
 
 struct TcEpilogue {
   const float* bias;      // [O] or null
@@ -40,13 +41,12 @@ struct TcEpilogue {
   int S, O, K;
   int relu;
   int gelu;  // exact (erf) GELU, torch.nn.functional.gelu default
-  int vec8;  // set by the launcher: Y / residual rows are 32-byte aligned -> 256-bit global accesses
   int pdl;          // launch with programmatic stream serialization (the kernel's prologue overlaps the previous kernel's tail)
   int allow_small;  // caller opts in to the small-problem regime below (split-K sums in arrival order: not bit-reproducible)
   // Small problems (fewer tiles than SMs), set by the launcher:
   int splits;  // split-K factor (>= 1).  > 1: Y already holds the residual (in-place residual stream); every split adds its
-               // partial product to it with vector reductions (red.global.add.v4.f32), split 0 also the bias.
-  int stats;   // 1: the folded-LayerNorm row statistics are computed inside the kernel, by the epilogue warps, from the X
+               // partial product to it with vector reductions (red.global.add.v2.f32), split 0 also the bias.
+  int stats;   // 1: the folded-LayerNorm row statistics are computed inside the kernel, by the consumer warpgroups, from the X
                // operand tiles as they pass through shared memory (row_mean / row_rstd are not read); needs splits == 1
 };
 
@@ -59,61 +59,93 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
                "l"(map), "r"(bar), "r"(c0), "r"(c1)
                : "memory");
 }
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_100 UMMA): start address >> 4, LBO unused (1), SBO = 8 rows x
-// 128 B = 1024 B between core-matrix groups, descriptor version 1, layout type 2 = SWIZZLE_128B.
-__device__ __forceinline__ uint64_t umma_desc_k128(uint32_t smem_addr) {
+// K-major, SWIZZLE_128B shared-memory matrix descriptor (sm_90 wgmma): start address >> 4 (bits 0-13), LBO unused (1),
+// SBO = 8 rows x 128 B = 1024 B between core-matrix groups (bits 32-45), base offset 0 (every tile is 1024-byte aligned),
+// layout type 1 = SWIZZLE_128B (bits 62-63).
+__device__ __forceinline__ uint64_t wgmma_desc_k128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// kind::tf32 instruction descriptor: D = F32 (bits 4-5 = 1), A/B = TF32 (2) K-major, N >> 3 at bit 17, M >> 4 at bit 24.
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kPending>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory");
 }
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+// D[64 x N] (+)= A[64 x 8] * B[N x 8]^T, TF32 products, fp32 accumulate; `accumulate` == 0 overwrites D.  Accumulator
+// fragment of thread t of the warpgroup: d[4i + 2h + e] = D[16 (t / 32) + (t % 32) / 4 + 8h][8i + 2 (t % 4) + e].
+__device__ __forceinline__ void wgmma_tf32(float (&d)[16], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "%16, %17, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate)
       : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
+__device__ __forceinline__ void wgmma_tf32(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate)
       : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+}
+__device__ __forceinline__ void wgmma_tf32(float (&d)[48], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
+      "%48, %49, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate)
+      : "memory");
+}
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate)
+      : "memory");
 }
 
-__device__ __forceinline__ void ld_global_v8(const float* p, float (&r)[8]) {
-  asm volatile("ld.global.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(r[0]), "=f"(r[1]), "=f"(r[2]), "=f"(r[3]), "=f"(r[4]), "=f"(r[5]), "=f"(r[6]), "=f"(r[7])
-               : "l"(p)
-               : "memory");
-}
-__device__ __forceinline__ void st_global_v8(float* p, const float (&r)[8]) {
-  asm volatile("st.global.v8.f32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "f"(r[0]), "f"(r[1]), "f"(r[2]), "f"(r[3]), "f"(r[4]), "f"(r[5]),
-               "f"(r[6]), "f"(r[7])
-               : "memory");
-}
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void red_add_v4(float* p, float a, float b, float c, float d) {
-  asm volatile("red.relaxed.gpu.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+__device__ __forceinline__ void red_add_v2(float* p, float a, float b) {
+  asm volatile("red.relaxed.gpu.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");
 }
 __device__ __forceinline__ float4 lds_f4(uint32_t addr) {
   float4 v;
@@ -121,15 +153,14 @@ __device__ __forceinline__ float4 lds_f4(uint32_t addr) {
   return v;
 }
 
-// Persistent: every CTA walks the work list (work = blockIdx.x, + gridDim.x, ...; work = split * tiles + tile, feature-tile index
-// fastest so that CTAs running side by side share the same 128 token rows in L2; split s of E.splits covers the k-blocks
-// [s, s+1) * K/32 / splits).  The accumulator is double buffered in TMEM (2 x BN columns): while the four
-// epilogue warps drain tile i, the TMA and MMA warps are already inside tile i+1.
+// Persistent: every CTA walks the work list (work = blockIdx.x, + gridDim.x, ...; work = split * tiles + tile, N-side tile index
+// fastest so that CTAs running side by side share the same 128 M-side rows in L2; split s of E.splits covers the k-blocks
+// [s, s+1) * K/32 / splits).  The ring is shared by the two consumer warpgroups: a stage is released once all 8 consumer
+// warps have retired the MMAs that read it (and, with E.stats, read its X rows).
 template <int BN, int ST = kTcStages, bool kSwap = false>
 __global__ void __launch_bounds__(kTcThreads, 1)
 tc_linear_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w, const TcEpilogue E) {
   static_assert(kSwap ? (BN == 32 || BN == 64 || BN == 96) : (BN == 64 || BN == 128), "N-side tile");
-  constexpr uint32_t kTmemCols = (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : 256;  // two accumulators, power of two >= 32
   extern __shared__ unsigned char tc_smem_raw[];
   const uint32_t raw = smem_u32(tc_smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;  // SWIZZLE_128B tiles need 1024-byte alignment
@@ -137,11 +168,6 @@ tc_linear_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
   const uint32_t bar_base = base + ST * kStageBytes;
   auto full_bar = [&](int s) { return bar_base + s * 8; };
   auto empty_bar = [&](int s) { return bar_base + (ST + s) * 8; };
-  auto tmem_full_bar = [&](int b) { return bar_base + (2 * ST + b) * 8; };
-  auto tmem_empty_bar = [&](int b) { return bar_base + (2 * ST + 2 + b) * 8; };
-  const uint32_t tmem_slot = bar_base + (2 * ST + 4) * 8;
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(tc_smem_raw + (tmem_slot - raw));
 
   pdl_trigger();  // the next kernel of a programmatic chain may start its own prologue now (it still waits for our completion)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -154,31 +180,20 @@ tc_linear_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
   const int total_work = total_tiles * splits;
   const bool stats = !kSwap && E.stats && splits == 1;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
     for (int s = 0; s < ST; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), stats ? 1 + 4 : 1);  // MMA commit (+ one arrival per epilogue warp that read the X tile for the row statistics)
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(tmem_full_bar(b), 1);
-      mbar_init(tmem_empty_bar(b), 4 * 32);  // every epilogue thread arrives once it has read its part of the buffer
+      mbar_init(empty_bar(s), kTcConsumerWarps);
     }
     mbar_fence_init();
   }
-  if (warp == 1) {  // TMEM allocation: two BN-column fp32 accumulators (power of two >= 32)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(kTmemCols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_acc = *tmem_slot_ptr;
-  pdl_wait();  // everything above touched only this CTA's shared memory / TMEM; global reads and writes start below
+  pdl_wait();  // everything above touched only this CTA's shared memory; global reads and writes start below
 
-  if (warp == 0) {
-    if (lane == 0) {  // ===== TMA producer =====
+  if (warp < 4) {
+    if (threadIdx.x == 0) {  // ===== TMA producer =====
       int it = 0;
       for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
         const int tile = work % total_tiles, split = work / total_tiles;
@@ -194,87 +209,81 @@ tc_linear_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {  // ===== MMA issuer =====
-      const uint32_t idesc = umma_idesc_tf32(kTcBM, BN);
-      int it = 0, lt = 0;
-      for (int work = blockIdx.x; work < total_work; work += gridDim.x, ++lt) {
-        const int split = work / total_tiles;
-        const int kb0 = split * num_kb / splits, kb1 = (split + 1) * num_kb / splits;
-        const int buf = lt & 1;
-        mbar_wait(tmem_empty_bar(buf), ((lt >> 1) & 1) ^ 1);  // the epilogue has drained this buffer (passes at first use)
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t acc = tmem_acc + (uint32_t)(buf * BN);
-        for (int kb = kb0; kb < kb1; ++kb, ++it) {
-          const int s = it % ST;
-          const uint32_t ph = (it / ST) & 1;
-          mbar_wait(full_bar(s), ph);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint64_t da = umma_desc_k128(base + s * kStageBytes);
-          const uint64_t db = umma_desc_k128(base + s * kStageBytes + kABytes);
+    return;
+  }
+
+  // ===== consumers: warpgroup wg owns M-side rows [64 wg, 64 wg + 64) of every tile =====
+  const int wg = (warp >> 2) - 1, wq = warp & 3, t = threadIdx.x & 127;
+  const int q2 = 2 * (lane & 3);
+  const float* bias = E.bias;
+  if (bias && E.t_ptr) bias += (size_t)(*E.t_ptr) * E.bias_t_stride;
+  float acc[BN / 2] = {};
+  int it = 0;
+  for (int work = blockIdx.x; work < total_work; work += gridDim.x) {
+    const int tile = work % total_tiles, split = work / total_tiles;
+    const int m0 = (tile / n_tiles) * kTcBM, n0 = (tile % n_tiles) * BN;
+    const int kb0 = split * num_kb / splits, kb1 = (split + 1) * num_kb / splits;
+    // folded-LayerNorm statistics (stats): thread t sums half t & 1 of row t >> 1 of this warpgroup's 64 X rows.  A row is 128
+    // contiguous bytes of a stage (SWIZZLE_128B only permutes the 16-byte chunks inside it, and a sum does not care); the
+    // chunk order is rotated by row so that a warp's loads spread over all banks.  Shifted by the first value stored in the
+    // row, which both halves read (one-pass variance without cancellation).
+    float pivot = 0.f, s1 = 0.f, s2 = 0.f;
+    for (int kb = kb0; kb < kb1; ++kb, ++it) {
+      const int s = it % ST;
+      mbar_wait(full_bar(s), (it / ST) & 1);
+      const uint32_t a_tile = base + s * kStageBytes + (uint32_t)wg * (64 * 128);
+      const uint64_t da = wgmma_desc_k128(a_tile);
+      const uint64_t db = wgmma_desc_k128(base + s * kStageBytes + kABytes);
+      wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < kTcBK / 8; ++k)  // advance 8 floats = 32 bytes inside the swizzle atom: +2 in the (>>4) address field
-            umma_tf32(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, ((kb - kb0) | k) ? 1u : 0u);
-          umma_commit(empty_bar(s));  // frees the slot once the MMAs that read it have retired
+      for (int k = 0; k < kTcBK / 8; ++k)  // advance 8 floats = 32 bytes inside the swizzle atom: +2 in the (>>4) address field
+        wgmma_tf32(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb > kb0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      if (stats) {
+        const uint32_t rowaddr = a_tile + (uint32_t)(t >> 1) * 128u;
+        if (kb == kb0) pivot = lds_f4(rowaddr).x;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float4 x = lds_f4(rowaddr + (uint32_t)((((t & 1) << 2) | ((j + (t >> 1)) & 3)) << 4));
+          const float a = x.x - pivot, b = x.y - pivot, c = x.z - pivot, d = x.w - pivot;
+          s1 += (a + b) + (c + d);
+          s2 += (a * a + b * b) + (c * c + d * d);
         }
-        umma_commit(tmem_full_bar(buf));  // accumulator complete
+      }
+      wgmma_wait<1>();  // the MMAs of the previous stage have retired: hand that stage back to the producer
+      if (kb > kb0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_bar((it + ST - 1) % ST));
       }
     }
-  } else {  // ===== epilogue: warps 2..5, TMEM lane quarter = warp % 4 =====
-    const int quarter = warp & 3;
-    const float* bias = E.bias;
-    if (bias && E.t_ptr) bias += (size_t)(*E.t_ptr) * E.bias_t_stride;
-    int lt = 0, it = 0;
-    for (int work = blockIdx.x; work < total_work; work += gridDim.x, ++lt) {
-      const int tile = work % total_tiles, split = work / total_tiles;
-      const int m0 = (tile / n_tiles) * kTcBM, n0 = (tile % n_tiles) * BN;
-      const int buf = lt & 1;
-      // folded-LayerNorm statistics of this thread's token row, from the X tiles in the ring: a row is 128 contiguous bytes of a
-      // stage (SWIZZLE_128B only permutes the 16-byte chunks inside it, and a sum does not care); lane l starts at chunk l % 8 so
-      // that a warp's loads spread over all banks.  Shifted by the first value read (one-pass variance without cancellation).
-      float st_mean = 0.f, st_rstd = 1.f;
-      if (stats) {
-        float pivot = 0.f, s1 = 0.f, s2 = 0.f;
-        for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % ST;
-          mbar_wait(full_bar(s), (it / ST) & 1);
-          const uint32_t rowaddr = base + s * kStageBytes + (uint32_t)(quarter * 32 + lane) * 128u;
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty_bar((it + ST - 1) % ST));
+
+    float st_mean = 0.f, st_rstd = 1.f;  // statistics of row t >> 1 (both threads of the row hold them)
+    if (stats) {
+      s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
+      s2 += __shfl_xor_sync(0xffffffffu, s2, 1);
+      const float inv_k = 1.0f / (float)E.K;
+      const float m = s1 * inv_k;
+      st_mean = pivot + m;
+      st_rstd = 1.0f / sqrtf(fmaxf(s2 * inv_k - m * m, 0.f) + 1e-5f);
+    }
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 x = lds_f4(rowaddr + (uint32_t)(((j + lane) & 7) << 4));
-            if (kb == 0 && j == 0) pivot = x.x;
-            const float a = x.x - pivot, b = x.y - pivot, c = x.z - pivot, d = x.w - pivot;
-            s1 += (a + b) + (c + d);
-            s2 += (a * a + b * b) + (c * c + d * d);
-          }
-          __syncwarp();
-          if (lane == 0) mbar_arrive(empty_bar(s));
-        }
-        const float inv_k = 1.0f / (float)E.K;
-        const float m = s1 * inv_k;
-        st_mean = pivot + m;
-        st_rstd = 1.0f / sqrtf(fmaxf(s2 * inv_k - m * m, 0.f) + 1e-5f);
-      }
-      mbar_wait(tmem_full_bar(buf), (lt >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    for (int h = 0; h < 2; ++h) {
+      const int fr = 16 * wq + (lane >> 2) + 8 * h;  // fragment row inside the warpgroup's 64 rows
       if constexpr (kSwap) {
-        // accumulator row (TMEM lane) = feature o, column = token: one warp store covers 32 consecutive features of a token
-        const int o = m0 + quarter * 32 + lane;
+        // fragment row = feature o, column = token: 8 lanes store 8 consecutive features of a token (one 32-byte sector)
+        const int o = m0 + 64 * wg + fr;
         const float b_o = bias ? __ldg(bias + o) : 0.f;
         const float cs_o = E.colsum ? __ldg(E.colsum + o) : 0.f;
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 32) {
-          float v[32];
-          tmem_ld32(tmem_acc + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * BN + c0), v);
-          if (c0 + 32 == BN) {
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive(tmem_empty_bar(buf));
-          }
 #pragma unroll
-          for (int t = 0; t < 32; ++t) {
-            const int srow = n0 + c0 + t;
-            if (srow < E.S) {  // warp-uniform
-              float x = v[t];
+        for (int i = 0; i < BN / 8; ++i) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int srow = n0 + 8 * i + q2 + e;
+            if (srow < E.S) {
+              float x = acc[4 * i + 2 * h + e];
               if (E.colsum) x = __ldg(E.row_rstd + srow) * (x - __ldg(E.row_mean + srow) * cs_o);
               x += b_o;
               if (E.residual) x += E.residual[(size_t)srow * E.ldr + o];
@@ -284,79 +293,54 @@ tc_linear_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
             }
           }
         }
-        continue;
-      }
-      const int row = m0 + quarter * 32 + lane;
-      const bool row_ok = row < E.S;
-      float mean = st_mean, rstd = st_rstd;
-      if (E.colsum && row_ok && !stats) {
-        mean = E.row_mean[row];
-        rstd = E.row_rstd[row];
-      }
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        float v[32];
-        tmem_ld32(tmem_acc + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * BN + c0), v);
-        if (c0 + 32 == BN) {  // this thread's last read of the buffer: hand it back to the MMA warp before the global stores
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          mbar_arrive(tmem_empty_bar(buf));
+      } else {
+        // fragment row = token, columns = features: the 4 lanes of a quad store 8 consecutive features (one 32-byte sector)
+        const int row = m0 + 64 * wg + fr;
+        float mean = 0.f, rstd = 1.f;
+        if (stats) {  // the row's statistics live with thread 2 fr of this warpgroup: lane 2 fr % 32 of this warp
+          mean = __shfl_sync(0xffffffffu, st_mean, (2 * fr) & 31);
+          rstd = __shfl_sync(0xffffffffu, st_rstd, (2 * fr) & 31);
+        } else if (E.colsum && row < E.S) {
+          mean = E.row_mean[row];
+          rstd = E.row_rstd[row];
         }
-        if (row_ok) {
-          float* yrow = E.Y + (size_t)row * E.ldy + n0 + c0;
-          const float* rrow = E.residual ? E.residual + (size_t)row * E.ldr + n0 + c0 : nullptr;
-          // A thread owns one output row: 8 consecutive floats = one full 32-byte sector per access (256-bit LDG / STG), so
-          // the row-per-thread pattern at least never writes partial sectors (16-byte stores doubled the L2 write traffic).
+        if (row < E.S) {
+          float* yrow = E.Y + (size_t)row * E.ldy + n0 + q2;
+          const float* rrow = E.residual ? E.residual + (size_t)row * E.ldr + n0 + q2 : nullptr;
 #pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            float o[8];
-#pragma unroll
-            for (int t = 0; t < 8; ++t) {
-              const int col = n0 + c0 + j + t;
-              float x = v[j + t];
-              if (E.colsum) x = rstd * (x - mean * __ldg(E.colsum + col));
-              if (bias && split == 0) x += __ldg(bias + col);
-              o[t] = x;
+          for (int i = 0; i < BN / 8; ++i) {
+            const int col = n0 + 8 * i + q2;
+            float o0 = acc[4 * i + 2 * h], o1 = acc[4 * i + 2 * h + 1];
+            if (E.colsum) {
+              o0 = rstd * (o0 - mean * __ldg(E.colsum + col));
+              o1 = rstd * (o1 - mean * __ldg(E.colsum + col + 1));
+            }
+            if (bias && split == 0) {
+              o0 += __ldg(bias + col);
+              o1 += __ldg(bias + col + 1);
             }
             if (splits > 1) {  // Y holds the residual already: accumulate this split's partial product on top of it
-              red_add_v4(yrow + j, o[0], o[1], o[2], o[3]);
-              red_add_v4(yrow + j + 4, o[4], o[5], o[6], o[7]);
+              red_add_v2(yrow + 8 * i, o0, o1);
               continue;
             }
             if (rrow) {
-              float r[8];
-              if (E.vec8) {
-                ld_global_v8(rrow + j, r);
-              } else {
-                const float4 a = *reinterpret_cast<const float4*>(rrow + j), b = *reinterpret_cast<const float4*>(rrow + j + 4);
-                r[0] = a.x; r[1] = a.y; r[2] = a.z; r[3] = a.w; r[4] = b.x; r[5] = b.y; r[6] = b.z; r[7] = b.w;
-              }
-#pragma unroll
-              for (int t = 0; t < 8; ++t) o[t] += r[t];
+              const float2 r = *reinterpret_cast<const float2*>(rrow + 8 * i);
+              o0 += r.x;
+              o1 += r.y;
             }
             if (E.relu) {
-#pragma unroll
-              for (int t = 0; t < 8; ++t) o[t] = fmaxf(o[t], 0.f);
+              o0 = fmaxf(o0, 0.f);
+              o1 = fmaxf(o1, 0.f);
             }
             if (E.gelu) {
-#pragma unroll
-              for (int t = 0; t < 8; ++t) o[t] = 0.5f * o[t] * (1.0f + erff(o[t] * 0.70710678118654752f));
+              o0 = 0.5f * o0 * (1.0f + erff(o0 * 0.70710678118654752f));
+              o1 = 0.5f * o1 * (1.0f + erff(o1 * 0.70710678118654752f));
             }
-            if (E.vec8) {
-              st_global_v8(yrow + j, o);
-            } else {
-              *reinterpret_cast<float4*>(yrow + j) = make_float4(o[0], o[1], o[2], o[3]);
-              *reinterpret_cast<float4*>(yrow + j + 4) = make_float4(o[4], o[5], o[6], o[7]);
-            }
+            *reinterpret_cast<float2*>(yrow + 8 * i) = make_float2(o0, o1);
           }
         }
       }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  }
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_acc), "r"(kTmemCols) : "memory");
   }
 }
 

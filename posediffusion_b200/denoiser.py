@@ -1,5 +1,5 @@
 """`Denoiser` with the reference's constructor, parameter names and state_dict layout
-(models/denoiser.py:22-98), whose forward runs the hand-written sm_100a kernels.
+(models/denoiser.py:22-98), whose forward runs the hand-written sm_90a kernels.
 
 The torch modules below only HOLD the parameters (so real checkpoints load with strict=True and
 `.to(device)` works); no torch operator runs in `forward`.  The kernels are compiled for the checkpoint
@@ -62,7 +62,7 @@ class Denoiser(nn.Module):
         want = dict(d_model=512, nhead=4, dim_feedforward=1024, num_encoder_layers=8, norm_first=True, batch_first=True)
         if arch != want or target_dim != 9 or not pivot_cam_onehot or z_dim != 384 or mlp_hidden_dim != 128:
             raise NotImplementedError(
-                f"the sm_100a kernels are built for the checkpoint architecture {want} with target_dim=9, z_dim=384, "
+                f"the sm_90a kernels are built for the checkpoint architecture {want} with target_dim=9, z_dim=384, "
                 f"mlp_hidden_dim=128, pivot_cam_onehot=True; got {arch}"
             )
         self.pivot_cam_onehot = pivot_cam_onehot

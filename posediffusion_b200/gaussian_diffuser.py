@@ -33,7 +33,7 @@ class GaussianDiffusion(nn.Module):
         if beta_schedule == "custom":  # the released configuration (cfgs/default.yaml); models/gaussian_diffuser.py:66-69
             betas = torch.linspace(beta_1, beta_T, timesteps, dtype=torch.float64)
         elif beta_schedule in ("linear", "cosine"):
-            # the reference also offers these (:62-65); no released checkpoint uses them and the sm_100a sampler tabulates
+            # the reference also offers these (:62-65); no released checkpoint uses them and the sm_90a sampler tabulates
             # the custom schedule only -- refuse at construction instead of building buffers nothing can run
             raise NotImplementedError(f"beta_schedule={beta_schedule!r}: only the released 'custom' schedule is built")
         else:
@@ -80,7 +80,7 @@ class GaussianDiffusion(nn.Module):
     def _require_native(self):
         if not self._native_ok():
             raise NotImplementedError(
-                "the sm_100a sampler is built for the released configuration: Denoiser model, objective='pred_noise', "
+                "the sm_90a sampler is built for the released configuration: Denoiser model, objective='pred_noise', "
                 "beta_schedule='custom' (beta 1e-4..0.1), 100 timesteps"
             )
 
@@ -152,4 +152,4 @@ class GaussianDiffusion(nn.Module):
         return self.p_sample_loop(shape, z=z, cond_fn=cond_fn, cond_start_step=cond_start_step)
 
     def forward(self, *args, **kwargs):
-        raise NotImplementedError("training (p_losses) is outside the B200 sampling hot path")
+        raise NotImplementedError("training (p_losses) is outside the native sampling hot path")

@@ -1,5 +1,5 @@
 """`geometry_guided_sampling` with the reference's signature (util/geometry_guided_sampling.py:14),
-running all five GGS_optimize phases in one persistent sm_100a kernel launch.
+running all five GGS_optimize phases in one persistent sm_90a kernel launch.
 
     cond_fn = partial(geometry_guided_sampling, matches_dict=matches_dict, GGS_cfg=GGS_cfg)   # demo.py:89
     model_mean = cond_fn(model_mean, t)

@@ -3,7 +3,7 @@
 The backbone the reference downloads with `torch.hub.load("facebookresearch/dino:main", "dino_vits16")` is represented here by
 `DinoViTSmall16`, a parameter container with the hub checkpoint's names and shapes (so the released checkpoint's
 `image_feature_extractor._net.*` keys load strictly).  It has no PyTorch forward: features come from the native library
-(pdb_extract_features -- patch embedding, the 12 blocks and the head as tcgen05/TMA GEMMs + shared-memory attention).
+(pdb_extract_features -- patch embedding, the 12 blocks and the head as wgmma/TMA GEMMs + shared-memory attention).
 """
 from __future__ import annotations
 
@@ -74,7 +74,7 @@ class MultiScaleImageFeatureExtractor(nn.Module):
         self.scale_factors: List[float] = list(scale_factors)
         if modelname != "dino_vits16":
             if "res" in modelname or "dino" in modelname:
-                raise NotImplementedError(f"{modelname}: only dino_vits16 (cfgs/default.yaml) has a B200-native backbone")
+                raise NotImplementedError(f"{modelname}: only dino_vits16 (cfgs/default.yaml) has a native backbone")
             raise ValueError(f"Unknown model name {modelname}")  # image_feature_extractor.py:46-47
         self._net = DinoViTSmall16()
         self._output_dim = self._net.norm.weight.shape[0]

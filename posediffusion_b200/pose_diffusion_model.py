@@ -28,7 +28,7 @@ def instantiate(cfg, **overrides):
     spec = dict(cfg)
     name = spec.pop("_target_").rsplit(".", 1)[-1]
     if name not in _TARGETS:
-        raise NotImplementedError(f"_target_ {name} is outside the B200 sampling hot path")
+        raise NotImplementedError(f"_target_ {name} is outside the native sampling hot path")
     spec.update(overrides)
     return _TARGETS[name](**spec)
 
@@ -59,7 +59,7 @@ class PoseDiffusionModel(nn.Module):
     def forward(self, image: Optional[torch.Tensor] = None, gt_cameras=None, sequence_name: Optional[List[str]] = None,
                 cond_fn=None, cond_start_step=0, training=True, batch_repeat=-1, z: Optional[torch.Tensor] = None):
         if training:
-            raise NotImplementedError("training is outside the B200 sampling hot path; call with training=False")
+            raise NotImplementedError("training is outside the native sampling hot path; call with training=False")
         if z is None:
             if self.image_feature_extractor is None or image is None:
                 raise ValueError("no image feature extractor configured: pass precomputed features as z=[B,N,384]")

@@ -1,7 +1,7 @@
 """Synthetic inputs for the sampling hot path (bench + tests).
 
 There is no network for the Co3D checkpoint, DINO weights or hloc matches, so both
-the B200 path and the CPU oracle run on: random-init denoiser weights with the
+the native path and the CPU oracle run on: random-init denoiser weights with the
 reference's initialisation law (trunc-normal sigma=0.02 Linear weights, zero biases,
 unit LayerNorm; reference pose_diffusion_model.py:67-74), z ~ N(0,1) of DINO ViT-S/16
 CLS shape [B,N,384], pre-drawn Gaussian noise, and 2D correspondences in the

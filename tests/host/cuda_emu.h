@@ -39,7 +39,7 @@ namespace emu {
 
 constexpr int kWarp = 32;
 constexpr size_t kStackBytes = 2048 * 1024;
-constexpr size_t kSharedBytes = 232448;  // 227 KB opt-in maximum per CTA on sm_100
+constexpr size_t kSharedBytes = 232448;  // 227 KB opt-in maximum per CTA on sm_90
 
 struct Cta {
   int nthreads = 0, nwarps = 0;
@@ -163,9 +163,6 @@ inline float __int_as_float(int i) { float f; memcpy(&f, &i, 4); return f; }
 inline int __float_as_int(float f) { int i; memcpy(&i, &f, 4); return i; }
 inline float __uint_as_float(unsigned u) { float f; memcpy(&f, &u, 4); return f; }
 inline unsigned __float_as_uint(float f) { unsigned u; memcpy(&u, &f, 4); return u; }
-inline float2 __ffma2_rn(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
-inline float2 __fmul2_rn(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
-inline float2 __fadd2_rn(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 using std::max;
 using std::min;
 

@@ -1,5 +1,5 @@
 // TEST HARNESS (not product): runs the persistent kernels of posediffusion_b200/csrc -- the same sources nvcc compiles for
-// sm_100a -- on the CPU through the execution-model emulation of cuda_emu.h: the GGS kernel body (csrc/ggs.cuh, every
+// sm_90a -- on the CPU through the execution-model emulation of cuda_emu.h: the GGS kernel body (csrc/ggs.cuh, every
 // template variant and streaming mode), the fp32 denoiser kernel (csrc/denoiser.cuh) and the camera-alignment kernels
 // (csrc/align.cuh).  Build:  g++ -O1 -std=c++17 -shared -fPIC (see __graft_entry__.py::build_emulator).
 #include "cuda_emu.h"

@@ -1,5 +1,5 @@
-"""CPU-only checks of bench.py's contract: the reference arm (`--impl reference`: the reference's own modules from /root/reference
-or baseline/_ref when present, else the CPU oracle port, on the host cores) prints ONE JSON line with the keys the driver reads, non-zero ranks of a multi-process launch exit without work, and the b200 arm
+"""CPU-only checks of bench.py's contract: the reference arm (`--impl reference`: the reference's own modules from a reference
+checkout or oracle/_ref when present, else the CPU oracle port, on the host cores) prints ONE JSON line with the keys the driver reads, non-zero ranks of a multi-process launch exit without work, and the b200 arm
 refuses to run without a GPU instead of falling back."""
 import json
 import os
@@ -38,7 +38,7 @@ def test_reference_arm_prints_one_contract_line():
 
 
 def test_reference_arm_falls_back_to_the_port_without_the_reference(tmp_path):
-    """Neither /root/reference nor baseline/_ref: the arm times the oracle port and says so (`kind: "port"`)."""
+    """Neither a reference checkout nor oracle/_ref: the arm times the oracle port and says so (`kind: "port"`)."""
     res = run(["--impl", "reference", "--workload", "cfg1", "--gpus", "1", "--steps", "1", "--warmup", "1"],
               env={"POSEDIFF_REFERENCE_ROOT": str(tmp_path), "POSEDIFF_INSTALLED_REFERENCE": str(tmp_path)})
     assert res.returncode == 0, res.stderr[-2000:]

@@ -1,4 +1,4 @@
-"""CPU execution of the GGS KERNEL SOURCE (csrc/ggs.cuh, the file nvcc compiles for sm_100a) through the emulation of the CUDA
+"""CPU execution of the GGS KERNEL SOURCE (csrc/ggs.cuh, the file nvcc compiles for sm_90a) through the emulation of the CUDA
 execution model in tests/host/cuda_emu.h: every CUDA thread is a coroutine, warp collectives / block barriers / the mbarrier
 + bulk-copy ring / the grid-wide release-acquire barrier behave as on the device, CTAs run as concurrent OS threads.
 

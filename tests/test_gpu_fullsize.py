@@ -37,7 +37,7 @@ TRANSFORMER = dict(d_model=512, nhead=4, dim_feedforward=1024, num_encoder_layer
 
 @pytest.fixture(scope="module")
 def dev():
-    assert torch.cuda.is_available(), "GPU tests need a B200"
+    assert torch.cuda.is_available(), "GPU tests need an H100"
     return torch.device("cuda:0")
 
 
@@ -74,7 +74,7 @@ def check_eval(ctx, dev, m, start, ref, layout, flags=(True, True, True)):
 
 @pytest.mark.parametrize("layout", ["plain", "paired"])
 def test_sampson_eval_vs_f64_oracle_at_config3_size(ctx, dev, cfg3_scene, layout):
-    """778 240 matches: 148 CTAs, ~164 rounds per CTA staged in shared memory (the path the headline bench runs)."""
+    """778 240 matches: one CTA per SM, ~184 rounds per CTA on 132 SMs staged in shared memory (the path the headline bench runs)."""
     m, start, ref = cfg3_scene
     assert len(m["kp1"]) == 380 * 2048 and ref["n_valid"] > 300000
     check_eval(ctx, dev, m, start, ref, layout)

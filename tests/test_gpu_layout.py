@@ -24,7 +24,7 @@ FLAGS = ((1, 1, 1), (0, 0, 1), (1, 0, 0), (0, 1, 0))
 
 @pytest.fixture(scope="module")
 def dev():
-    assert torch.cuda.is_available(), "GPU tests need a B200"
+    assert torch.cuda.is_available(), "GPU tests need an H100"
     return torch.device("cuda:0")
 
 

@@ -1,4 +1,4 @@
-"""GPU parity tests: the sm_100a path (through the C-ABI library) vs the reference fixtures
+"""GPU parity tests: the sm_90a path (through the C-ABI library) vs the reference fixtures
 (tests/golden, produced by the reference's own modules) and vs the CPU oracle on seeded inputs.
 
 Tolerances (fp32 end to end; the reference is fp32 too):
@@ -29,7 +29,7 @@ FLAGS = ((1, 1, 1), (0, 0, 1), (1, 0, 0), (0, 1, 0))
 
 @pytest.fixture(scope="module")
 def dev():
-    assert torch.cuda.is_available(), "GPU tests need a B200"
+    assert torch.cuda.is_available(), "GPU tests need an H100"
     return torch.device("cuda:0")
 
 

@@ -1,4 +1,4 @@
-"""tcgen05 + TMA linear layer (csrc/tc_linear.cuh) vs a plain PyTorch fp32 matmul of the same op.
+"""wgmma + TMA linear layer (csrc/tc_linear.cuh) vs a plain PyTorch fp32 matmul of the same op.
 Tolerance: TF32 products (10-bit mantissa), fp32 accumulate -> 2e-3 of max |y| (stated; K <= 1024)."""
 import numpy as np
 import pytest
@@ -22,7 +22,7 @@ def swap_on(ctx, request):
     ctx.set_tc_swap(False)
 
 
-# with swap_on, S <= 96 and O % 128 == 0 takes the swap-AB instantiation (weights on the UMMA M side, 32 / 64 / 96 tokens on the N side)
+# with swap_on, S <= 96 and O % 128 == 0 takes the swap-AB instantiation (weights on the wgmma M side, 32 / 64 / 96 tokens on the N side)
 @pytest.mark.parametrize("S,O,K", [(128, 64, 32), (128, 512, 512), (160, 1536, 512), (20, 512, 1024), (300, 1024, 512), (1280, 512, 384),
                                    (5, 128, 512), (20, 1536, 512), (33, 512, 256), (64, 1024, 512), (80, 512, 1024), (96, 1536, 512),
                                    (20, 64, 512)])
@@ -67,7 +67,7 @@ TRANSFORMER = dict(d_model=512, nhead=4, dim_feedforward=1024, num_encoder_layer
 
 @pytest.mark.parametrize("B,N", [(8, 20), (1, 20), (2, 80), (1, 5), (1, 80), (3, 20), (7, 20), (32, 20), (50, 20)])
 def test_tensor_core_denoiser_engine_vs_fp32_engine_and_oracle(ctx, B, N, swap_on):
-    """The tcgen05/TMA engine (TF32 products, LayerNorm folded into the GEMM epilogue) against the exact-fp32 engine
+    """The wgmma/TMA engine (TF32 products, LayerNorm folded into the GEMM epilogue) against the exact-fp32 engine
     and the CPU oracle on the same inputs.  Tolerance 5e-3 absolute on eps (values O(0.1..1))."""
     import posediffusion_b200 as pdb
     from oracle import pose_oracle as po

@@ -3,7 +3,7 @@
 Written in a session without GPU access.  What was verified without a GPU: the device maths on the host (same __host__ __device__
 functions, tests/test_alignment_cpu.py), and the two kernel bodies on the CPU emulation of the execution model with the
 entry point's launch geometry (tests/host/cuda_emu.h).  The file sorts last among the GPU tests on purpose: it is the one
-test module whose kernels had not run on a B200 when it was committed.
+test module whose kernels ran last on the GPU when it was written.
 """
 import numpy as np
 import pytest

@@ -106,7 +106,7 @@ def _walk(harness, m, layout, mode, cpp, seed=0):
 
 @pytest.mark.parametrize("case", sorted(CASES))
 @pytest.mark.parametrize("mode", [0, 1, 2], ids=["resident", "ring", "stream"])
-@pytest.mark.parametrize("cpp", [1, 3, 148])
+@pytest.mark.parametrize("cpp", [1, 3, 132, 148])
 def test_kernel_traversal_consumes_every_match_once_in_both_layouts(harness, case, mode, cpp):
     m = CASES[case]()
     out = {}
@@ -123,12 +123,12 @@ def test_kernel_traversal_consumes_every_match_once_in_both_layouts(harness, cas
 
 
 def test_paired_layout_keeps_the_packed_fast_path_share_at_benchmark_shape(harness):
-    """At the headline shape (config 3: 20 frames, 2048 matches for each of the 380 ordered pairs, 148 CTAs) the paired walk
+    """At the headline shape (config 3: 20 frames, 2048 matches for each of the 380 ordered pairs, 132 CTAs = one per H100 SM) the paired walk
     must take the packed fast path at least as often as the plain one (otherwise the layout would trade MOVs for scalar tails)."""
     m = syn.uniform_matches(20, 2048, seed=5)
     for mode, floor in ((0, 0.99), (1, 0.75)):
-        _, _, _, f_plain = _walk(harness, m, "plain", mode, 148)
-        _, _, _, f_pair = _walk(harness, m, "paired", mode, 148)
+        _, _, _, f_plain = _walk(harness, m, "plain", mode, 132)
+        _, _, _, f_pair = _walk(harness, m, "paired", mode, 132)
         assert f_pair[0] >= f_plain[0]
         assert f_pair[0] >= floor * f_pair.sum()
 

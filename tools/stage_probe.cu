@@ -14,7 +14,7 @@
 // CTAs that produce nothing can fall behind the producers by more than the 4 rotating buffers; the probe therefore accepts
 // NEWER tags as well (the kernel cannot: there every reader of a buffer is, transitively, a dependency of its next writer).
 //
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a tools/stage_probe.cu -o build/stage_probe
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a tools/stage_probe.cu -o build/stage_probe
 //   build/stage_probe [rows=20] [producers=64] [iters=20000]
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>

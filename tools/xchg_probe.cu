@@ -12,7 +12,7 @@
 //   mode 2  LL, TWO levels: groups of S CTAs, the group leader sums its group's slots and publishes a group slot,
 //           every CTA then reads the G group slots
 //
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a tools/xchg_probe.cu -o build/xchg_probe
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a tools/xchg_probe.cu -o build/xchg_probe
 //   build/xchg_probe [words=148] [iters=20000]
 #include <cuda_runtime.h>
 #include <cstdint>
