@@ -20,6 +20,8 @@
  *                             matches on the host, poses back on the host)
  *   pdb_sample_loop_host_matches <- the same call starting from the reference's matches_dict arrays (demo.py:94-108:
  *                             extract_match output straight into the sampler); packing overlaps the unguided steps
+ *   pdb_images_preprocess_host <- load_and_preprocess_images after PIL decoding (util/load_img_folder.py: float conversion,
+ *                             centre crop, bilinear resize; demo.py:51, test.py:172)
  *
  * Conventions: plain pointers and sizes only (no torch types).  `*_dev` pointers are CUDA device pointers
  * on the context's device, `*_host` are host pointers, `stream` is a cudaStream_t passed as void*
@@ -246,6 +248,16 @@ int pdb_extract_features(pdb_context* ctx, const float* images_dev, int32_t n_im
 /* The same with host buffers: copies the images in, z out, synchronises the stream. */
 int pdb_extract_features_host(pdb_context* ctx, const float* images_host, int32_t n_images, int32_t height, int32_t width,
                               const double* scale_factors, int32_t n_scales, float* z_host, void* stream);
+
+/* ---- image preprocessing ----------------------------------------------------------------------------
+ * load_and_preprocess_images (util/load_img_folder.py) after decoding: frame i is rgb_host[i], HOST uint8 HWC of
+ * hw[i] = {H, W} with row pitch 3*W (frames may differ in size); crop[i] = {top, left, side} is its square crop.
+ * images_dev [n,3,out_size,out_size] receives crop / 255 (IEEE division) resized bilinearly (align_corners=False, no antialias;
+ * ATen's CPU index and weight arithmetic, so a crop with side == out_size is copied exactly).  Only the crop columns of the rows
+ * the resize reads are uploaded.  Synchronises the stream before returning, so the frames may be freed afterwards.
+ * PDB_ERR_INVALID for n <= 0, out_size <= 0, a NULL pointer, or a crop outside its image or with side < 2. */
+int pdb_images_preprocess_host(pdb_context* ctx, int32_t n, const uint8_t* const* rgb_host, const int32_t* hw,
+                               const int32_t* crop, int32_t out_size, float* images_dev, void* stream);
 
 /* ---- post-loop geometry (widened row, SURVEY 8f-3) -----------------------------------------------
  * pose_encoding_to_camera for "absT_quaR_logFL" (util/camera_transform.py:64-105): pose_dev [count,9] -> R_dev [count,3,3]

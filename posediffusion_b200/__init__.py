@@ -11,9 +11,11 @@ from .denoiser import Denoiser, TransformerEncoderWrapper
 from .gaussian_diffuser import GaussianDiffusion
 from .geometry_guided_sampling import geometry_guided_sampling, invalidate_matches
 from .image_feature_extractor import MultiScaleImageFeatureExtractor
+from .load_img_folder import load_and_preprocess_images
 from .pose_diffusion_model import PoseDiffusionModel
 
 __all__ = [
     "PoseDiffusionModel", "GaussianDiffusion", "Denoiser", "TransformerEncoderWrapper", "MultiScaleImageFeatureExtractor",
     "geometry_guided_sampling", "invalidate_matches", "pose_encoding_to_camera", "PerspectiveCameras", "corresponding_cameras_alignment",
+    "load_and_preprocess_images",
 ]

@@ -98,6 +98,7 @@ EXPORTS = {
     "pdb_extract_features_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_double), C.c_int32, C.c_void_p, C.c_void_p]),
     "pdb_sample_loop_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p), C.c_int32, C.POINTER(GgsConfig), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pdb_sample_loop_host_matches": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_int32, C.c_int32, C.POINTER(GgsConfig), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pdb_images_preprocess_host": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None
@@ -418,6 +419,26 @@ class Context:
             self._ok(self.lib.pdb_extract_features_host(self.handle, images.ctypes.data_as(C.c_void_p), n, H, W, sf, len(scale_factors),
                                                         z.ctypes.data_as(C.c_void_p), _stream_ptr(self.device)), "pdb_extract_features_host")
         return z
+
+    def preprocess_images(self, frames: Sequence[np.ndarray], crops: Sequence[Sequence[int]], out_size: int) -> torch.Tensor:
+        """Decoded frames (uint8 [H,W,3] each, sizes may differ) and their square crops {top, left, side} -> float32
+        [n,3,out_size,out_size] on this device: crop / 255 resized bilinearly (pdb_images_preprocess_host)."""
+        keep = [np.ascontiguousarray(f, dtype=np.uint8) for f in frames]
+        for i, f in enumerate(keep):
+            if f.ndim != 3 or f.shape[2] != 3:
+                raise NativeError(f"frame {i} has shape {f.shape}, expected [H, W, 3] uint8")
+        n = len(keep)
+        ptrs = (C.c_void_p * max(n, 1))(*[f.ctypes.data for f in keep])
+        hw = np.asarray([f.shape[:2] for f in keep] or np.zeros((0, 2)), dtype=np.int32).reshape(-1, 2)
+        crop = np.ascontiguousarray(np.asarray(crops, dtype=np.int32).reshape(-1, 3))
+        if len(crop) != n:
+            raise NativeError(f"{len(crop)} crops for {n} frames")
+        images = torch.empty((n, 3, max(int(out_size), 0), max(int(out_size), 0)), device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            self._ok(self.lib.pdb_images_preprocess_host(self.handle, n, ptrs, hw.ctypes.data, crop.ctypes.data, int(out_size),
+                                                         C.c_void_p(images.data_ptr()), _stream_ptr(self.device)),
+                     "pdb_images_preprocess_host")
+        return images
 
     # ---- denoiser / sampler -----------------------------------------------------------------------
     def denoiser_forward(self, x: torch.Tensor, t: int, z: torch.Tensor) -> torch.Tensor:

@@ -280,6 +280,11 @@ void pdb_destroy(pdb_context* c) {
   if (ctx->pack_stream) cudaStreamDestroy(ctx->pack_stream);
   for (auto& b : ctx->pool) cudaFree(b.first);
   if (ctx->pin) cudaFreeHost(ctx->pin);
+  for (int s = 0; s < 2; ++s) {
+    if (ctx->pre_pin[s]) cudaFreeHost(ctx->pre_pin[s]);
+    if (ctx->pre_ev[s]) cudaEventDestroy(ctx->pre_ev[s]);
+  }
+  if (ctx->pre_dev) cudaFree(ctx->pre_dev);
   if (ctx->ggs_clock) cudaFree(ctx->ggs_clock);
   delete ctx;
 }

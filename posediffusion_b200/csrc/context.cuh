@@ -69,6 +69,13 @@ struct Context {
   // staging for the host-buffer entry point
   void* stage = nullptr;
   size_t stage_bytes = 0;
+  // image preprocessing (csrc/api_pre.cu): two pinned staging slots, the event of each slot's last upload, and the device copy
+  // of every frame's touched rows
+  void* pre_pin[2] = {nullptr, nullptr};
+  size_t pre_pin_bytes[2] = {0, 0};
+  cudaEvent_t pre_ev[2] = {nullptr, nullptr};
+  void* pre_dev = nullptr;
+  size_t pre_dev_bytes = 0;
 
   int fail(int code, const char* fmt, ...) {
     char buf[512];
