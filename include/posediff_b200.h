@@ -282,6 +282,34 @@ int pdb_cameras_align(pdb_context* ctx, const float* R_src_dev, const float* T_s
                       const float* T_tgt_dev, int32_t count, int32_t estimate_scale, double eps, float* R_out_dev,
                       float* T_out_dev, float* align_dev, void* stream);
 
+/* ---- training (GaussianDiffusion.p_losses + Denoiser, models/gaussian_diffuser.py:308-341) -----------------------------------
+ * params[108] are the denoiser parameters in pdb_denoiser_load order, device fp32, contiguous, 16-byte aligned; they are read
+ * directly on every call (only `_first.weight`, whose 702-float rows TMA cannot address, is copied into the workspace padded to
+ * 704 columns).  The workspace (pdb_train_workspace_bytes, device, 16-byte aligned) is owned by the caller: the forward writes
+ * the activations the backward needs into it, the backward also uses it as scratch.  At most 64 frames per sequence.
+ * Dropout: element e of site s (0 attention weights, 1 after out-proj, 2 after ReLU, 3 after linear2) of layer l is kept when
+ * Philox4x32-10(key = seed, counter = {e >> 2, e >> 34, l << 8 | s, 0}) word e & 3 >= floor(p * 2^32); kept values are scaled by
+ * 1 / (1 - p).  Elements are numbered row-major over [batch, heads, frames, frames] (site 0) and [batch * frames, width]. */
+int64_t pdb_train_workspace_bytes(int32_t batch, int32_t frames); /* 0 for an unsupported shape */
+/* x_start, noise [B,N,9]; t_dev [B] int32 in [0,100); z [B,N,384]; loss_type 0 = l1, 1 = l2.  Writes x_t = q_sample(x_start, t, noise),
+ * loss [B,N,9] (reduction none, against the noise) and x0 = predict_start_from_noise(x_t, t, eps).  The caller validates t: a value
+ * outside [0,100) is clamped where the kernels index the schedule (no out-of-bounds read), its outputs are meaningless, and
+ * pdb_train_backward on that workspace fails with PDB_ERR_INVALID. */
+int pdb_train_forward(pdb_context* ctx, const float* const* params, const float* x_start_dev, const int32_t* t_dev, const float* noise_dev,
+                      const float* z_dev, int32_t batch, int32_t frames, float dropout_p, uint64_t seed, int32_t loss_type, void* workspace,
+                      float* loss_dev, float* x_t_dev, float* x0_dev, void* stream);
+/* grads[108] (device, parameter shapes) are overwritten with d(sum(grad_loss * loss) + sum(grad_x0 * x0)) / d params; grad_loss or
+ * grad_x0 may be NULL (zero).  Synchronises the stream once to read the workspace header (shape, loss type, dropout seed, the
+ * timestep flag).  Bit-reproducible: no floating-point atomics. */
+int pdb_train_backward(pdb_context* ctx, const float* const* params, void* workspace, const float* grad_loss_dev, const float* grad_x0_dev,
+                       float* const* grads, void* stream);
+/* camera_to_pose_encoding, "absT_quaR_logFL" (util/camera_transform.py:108-129): R [count,3,3], T [count,3], focal [count,2] ->
+ * pose [count,9] = T | matrix_to_quaternion(R) with the real part made non-negative | log(clamp(focal, min, max)) - bias. */
+int pdb_camera_to_pose(pdb_context* ctx, const float* R_dev, const float* T_dev, const float* focal_dev, int32_t count,
+                       double log_focal_length_bias, double min_focal_length, double max_focal_length, float* pose_dev, void* stream);
+/* HOST-ONLY: out[i] = 1 if element offset + i of (layer, site) is kept under the dropout rule above, else 0. */
+int pdb_dropout_mask_host(uint64_t seed, int32_t layer, int32_t site, int64_t offset, int64_t count, float dropout_p, uint8_t* out);
+
 #ifdef __cplusplus
 }
 #endif

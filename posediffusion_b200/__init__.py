@@ -6,7 +6,7 @@ Public surface mirrors the reference's (`models.PoseDiffusionModel`, `models.Gau
 `libposediff_b200.so` (include/posediff_b200.h).  No CPU or PyTorch-operator fallback exists.
 """
 from .camera_alignment import corresponding_cameras_alignment
-from .camera_transform import PerspectiveCameras, pose_encoding_to_camera
+from .camera_transform import PerspectiveCameras, camera_to_pose_encoding, pose_encoding_to_camera
 from .denoiser import Denoiser, TransformerEncoderWrapper
 from .gaussian_diffuser import GaussianDiffusion
 from .geometry_guided_sampling import geometry_guided_sampling, invalidate_matches
@@ -16,6 +16,6 @@ from .pose_diffusion_model import PoseDiffusionModel
 
 __all__ = [
     "PoseDiffusionModel", "GaussianDiffusion", "Denoiser", "TransformerEncoderWrapper", "MultiScaleImageFeatureExtractor",
-    "geometry_guided_sampling", "invalidate_matches", "pose_encoding_to_camera", "PerspectiveCameras", "corresponding_cameras_alignment",
+    "geometry_guided_sampling", "invalidate_matches", "pose_encoding_to_camera", "camera_to_pose_encoding", "PerspectiveCameras", "corresponding_cameras_alignment",
     "load_and_preprocess_images",
 ]

@@ -99,7 +99,33 @@ EXPORTS = {
     "pdb_sample_loop_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p), C.c_int32, C.POINTER(GgsConfig), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pdb_sample_loop_host_matches": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_int32, C.c_int32, C.POINTER(GgsConfig), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pdb_images_preprocess_host": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "pdb_train_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32]),
+    "pdb_train_forward": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                    C.c_float, C.c_uint64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pdb_train_backward": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p]),
+    "pdb_camera_to_pose": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_double, C.c_double, C.c_double,
+                                     C.c_void_p, C.c_void_p]),
+    "pdb_dropout_mask_host": (C.c_int, [C.c_uint64, C.c_int32, C.c_int32, C.c_int64, C.c_int64, C.c_float, C.c_void_p]),
 }
+
+TRAIN_MAX_FRAMES = 64
+LOSS_TYPES = {"l1": 0, "l2": 1}
+DROPOUT_SITES = {"attn": 0, "out_proj": 1, "relu": 2, "linear2": 3}
+
+
+def dropout_mask_host(seed: int, layer: int, site: int, offset: int, count: int, p: float) -> np.ndarray:
+    """Keep mask (uint8, 1 = kept) of `count` elements from `offset` of dropout site `site` of layer `layer`: the same Philox
+    function the training kernels evaluate (no GPU needed)."""
+    out = np.zeros(max(int(count), 0), dtype=np.uint8)
+    rc = load_library().pdb_dropout_mask_host(int(seed) & (2**64 - 1), int(layer), int(site), int(offset), int(count), float(p),
+                                              out.ctypes.data_as(C.c_void_p))
+    if rc != 0:
+        raise ValueError(f"pdb_dropout_mask_host rejected (layer={layer}, site={site}, offset={offset}, count={count}, p={p})")
+    return out
+
+
+def train_workspace_bytes(batch: int, frames: int) -> int:
+    return int(load_library().pdb_train_workspace_bytes(int(batch), int(frames)))
 
 _lib = None
 _lib_lock = threading.Lock()
@@ -322,6 +348,64 @@ class Context:
         arr = (C.c_void_p * len(keep))(*[C.c_void_p(t.data_ptr()) for t in keep])
         with torch.cuda.device(self.device):
             self._ok(self.lib.pdb_denoiser_load(self.handle, arr, len(keep), _stream_ptr(self.device)), "pdb_denoiser_load")
+
+    # ---- training ------------------------------------------------------------------------------------
+    def _param_array(self, tensors: Sequence[torch.Tensor]):
+        if len(tensors) != PDB_NUM_WEIGHT_TENSORS:
+            raise NativeError(f"expected {PDB_NUM_WEIGHT_TENSORS} tensors, got {len(tensors)}")
+        for i, p in enumerate(tensors):
+            _check_dev(p, f"parameter {i}", self.device)
+        return (C.c_void_p * len(tensors))(*[C.c_void_p(p.data_ptr()) for p in tensors])
+
+    def train_forward(self, params: Sequence[torch.Tensor], x_start, t, noise, z, dropout_p: float, seed: int, loss_type: str):
+        """p_losses forward: returns (workspace, loss, x_t, x0).  The workspace holds what train_backward needs; it belongs to
+        the caller (one per outstanding forward)."""
+        B, N, _ = x_start.shape
+        for name, v, shape in (("x_start", x_start, (B, N, TARGET_DIM)), ("noise", noise, (B, N, TARGET_DIM)), ("z", z, (B, N, Z_DIM))):
+            _check_dev(v, name, self.device, shape)
+        if t.dtype != torch.int32 or tuple(t.shape) != (B,) or t.device != self.device or not t.is_contiguous():
+            raise NativeError(f"t must be a contiguous int32 [{B}] tensor on {self.device}")
+        if N > TRAIN_MAX_FRAMES:
+            raise NativeError(f"training supports at most {TRAIN_MAX_FRAMES} frames per sequence, got {N}")
+        nbytes = train_workspace_bytes(B, N)
+        ws = torch.empty(nbytes // 4, dtype=torch.float32, device=self.device)
+        loss, x_t, x0 = torch.empty_like(x_start), torch.empty_like(x_start), torch.empty_like(x_start)
+        arr = self._param_array(params)
+        with torch.cuda.device(self.device):
+            self._ok(self.lib.pdb_train_forward(self.handle, arr, x_start.data_ptr(), t.data_ptr(), noise.data_ptr(), z.data_ptr(), B, N,
+                                                float(dropout_p), int(seed) & (2**64 - 1), LOSS_TYPES[loss_type], ws.data_ptr(),
+                                                loss.data_ptr(), x_t.data_ptr(), x0.data_ptr(), _stream_ptr(self.device)),
+                     "pdb_train_forward")
+        return ws, loss, x_t, x0
+
+    def train_backward(self, params: Sequence[torch.Tensor], ws: torch.Tensor, grad_loss: Optional[torch.Tensor],
+                       grad_x0: Optional[torch.Tensor]) -> List[torch.Tensor]:
+        arr = self._param_array(params)
+        grads = [torch.empty_like(p) for p in params]
+        garr = (C.c_void_p * len(grads))(*[C.c_void_p(g.data_ptr()) for g in grads])
+        with torch.cuda.device(self.device):
+            self._ok(self.lib.pdb_train_backward(self.handle, arr, ws.data_ptr(),
+                                                 grad_loss.data_ptr() if grad_loss is not None else None,
+                                                 grad_x0.data_ptr() if grad_x0 is not None else None, garr, _stream_ptr(self.device)),
+                     "pdb_train_backward")
+        return grads
+
+    def camera_to_pose(self, R: torch.Tensor, T: torch.Tensor, focal: torch.Tensor, log_focal_length_bias=1.8, min_focal_length=0.1,
+                       max_focal_length=20.0) -> torch.Tensor:
+        """R [..., 3, 3], T [..., 3], focal [..., 2] -> pose [..., 9] (absT_quaR_logFL)."""
+        lead = tuple(T.shape[:-1])
+        Rf = R.reshape(-1, 3, 3).to(torch.float32).contiguous()
+        Tf = T.reshape(-1, 3).to(torch.float32).contiguous()
+        Ff = focal.reshape(-1, 2).to(torch.float32).contiguous()
+        n = Tf.shape[0]
+        for v, name, shape in ((Rf, "R", (n, 3, 3)), (Tf, "T", (n, 3)), (Ff, "focal_length", (n, 2))):
+            _check_dev(v, name, self.device, shape)
+        pose = torch.empty((n, TARGET_DIM), device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            self._ok(self.lib.pdb_camera_to_pose(self.handle, Rf.data_ptr(), Tf.data_ptr(), Ff.data_ptr(), n, float(log_focal_length_bias),
+                                                 float(min_focal_length), float(max_focal_length), pose.data_ptr(),
+                                                 _stream_ptr(self.device)), "pdb_camera_to_pose")
+        return pose.reshape(*lead, TARGET_DIM)
 
     # ---- post-loop geometry ---------------------------------------------------------------------------
     def pose_to_camera(self, pose: torch.Tensor, log_focal_length_bias=1.8, min_focal_length=0.1, max_focal_length=20.0):

@@ -49,6 +49,30 @@ class TimeStepEmbedding(nn.Module):
         self.linear = nn.Sequential(nn.Linear(dim, dim // 2), nn.SiLU(), nn.Linear(dim // 2, dim // 2))
 
 
+class _DiffusionLoss(torch.autograd.Function):
+    """Native p_losses: forward (pdb_train_forward) saves its activations in a workspace tensor that this graph node owns; backward
+    (pdb_train_backward) returns the gradients of the 108 parameters.  The parameters are saved for backward, so changing one in
+    place between the two raises torch's version error."""
+
+    @staticmethod
+    def forward(fctx, ctx, args, dropout_p, seed, loss_type, *params):
+        ws, loss, x_t, x0 = ctx.train_forward(params, *args, dropout_p, seed, loss_type)
+        fctx.native, fctx.ws = ctx, ws
+        fctx.save_for_backward(*params)
+        fctx.mark_non_differentiable(x_t)
+        return loss, x0, x_t
+
+    @staticmethod
+    def backward(fctx, grad_loss, grad_x0, _grad_x_t):
+        params = fctx.saved_tensors
+        if fctx.ws is None:
+            raise RuntimeError("the native training graph was already backpropagated and its workspace released")
+        grads = fctx.native.train_backward(params, fctx.ws, None if grad_loss is None else grad_loss.contiguous(),
+                                           None if grad_x0 is None else grad_x0.contiguous())
+        fctx.ws = None
+        return (None, None, None, None, None, *grads)
+
+
 class Denoiser(nn.Module):
     def __init__(self, TRANSFORMER: Dict, target_dim: int = 9, pivot_cam_onehot: bool = True, z_dim: int = 384,
                  mlp_hidden_dim: int = 128):
@@ -75,6 +99,7 @@ class Denoiser(nn.Module):
             nn.Linear(arch["d_model"], mlp_hidden_dim), nn.LayerNorm(mlp_hidden_dim), nn.ReLU(inplace=True),
             nn.Linear(mlp_hidden_dim, target_dim),
         )
+        self.dropout_p = float(_cfg_get(TRANSFORMER, "dropout", 0.1))  # applied by the training kernels in train() mode only
         self._native_token = _native.module_token()  # identity for the context's weight cache (never reused, unlike id())
         self._native_epoch = 0
 
@@ -99,6 +124,29 @@ class Denoiser(nn.Module):
     def invalidate_native_weights(self) -> None:
         """Force a re-upload at the next call (needed after editing parameters through `.data`, which does not bump `_version`)."""
         self._native_epoch += 1
+
+    def train_step_forward(self, x_start, t, noise, z, dropout_p: float, seed, loss_type: str):
+        """(loss, x_0_pred, x_t) of GaussianDiffusion.p_losses with autograd into this module's parameters (_DiffusionLoss).
+        `seed` is the 64-bit dropout seed, an int or a one-element integer tensor; timesteps outside [0, 100) raise IndexError."""
+        params = self.ordered_parameters()
+        device = params[0].device
+        if device.type != "cuda":
+            raise _native.NativeError("Denoiser parameters are on the CPU: call .to('cuda') (no CPU fallback)")
+        if torch.is_grad_enabled() and (x_start.requires_grad or z.requires_grad or noise.requires_grad):
+            raise NotImplementedError("gradients reach the denoiser parameters only: x_start, noise and z must not require grad "
+                                      "(train with a frozen image feature extractor)")
+        # t out of range and the seed (an int, or a one-element int64 tensor drawn on the device) in one device-to-host read
+        bad = ((t < 0) | (t >= _native.NUM_TIMESTEPS)).any().view(1).to(torch.int64)
+        if torch.is_tensor(seed):
+            seed_v, bad_v = torch.cat([seed.reshape(1).to(bad.device, torch.int64), bad]).tolist()
+        else:
+            seed_v, bad_v = int(seed), int(bad.item())
+        if bad_v:
+            raise IndexError(f"timesteps must lie in [0, {_native.NUM_TIMESTEPS})")
+        ctx = _native.Context.get(device)
+        args = (x_start.detach().contiguous().float(), t.to(torch.int32).contiguous(), noise.detach().contiguous().float(),
+                z.detach().contiguous().float())
+        return _DiffusionLoss.apply(ctx, args, float(dropout_p), seed_v, loss_type, *params)
 
     def forward(self, x: torch.Tensor, t: torch.Tensor, z: torch.Tensor) -> torch.Tensor:
         """x [B,N,9], t [B] (all entries equal, as the sampler passes them), z [B,N,384] -> eps [B,N,9]."""

@@ -1,6 +1,7 @@
 """`GaussianDiffusion` sampler with the reference's surface (models/gaussian_diffuser.py:75-306):
 same constructor, the same 13 persistent schedule buffers, `.model` attached after construction,
-`sample` / `p_sample_loop` / `p_sample`.  Training methods (q_sample, p_losses, forward) are out of scope.
+`sample` / `p_sample_loop` / `p_sample`, and the training methods `q_sample` / `p_losses` / `forward` (:211-216, :308-341),
+whose loss and gradients come from the native training kernels (csrc/api_train.cu).
 
 `p_sample_loop` runs the whole loop natively (one persistent denoiser launch for the unguided prefix, then
 denoiser + GGS launches per guided step) when `cond_fn` is None or a `partial(geometry_guided_sampling, ...)`
@@ -151,5 +152,42 @@ class GaussianDiffusion(nn.Module):
     def sample(self, shape, z, cond_fn=None, cond_start_step=0):
         return self.p_sample_loop(shape, z=z, cond_fn=cond_fn, cond_start_step=cond_start_step)
 
-    def forward(self, *args, **kwargs):
-        raise NotImplementedError("training (p_losses) is outside the native sampling hot path")
+    # ---- training (models/gaussian_diffuser.py:211-216, 308-341) ------------------------------------------
+    def _extract(self, a: torch.Tensor, t: torch.Tensor, x_shape) -> torch.Tensor:
+        return a.gather(-1, t).reshape(t.shape[0], *((1,) * (len(x_shape) - 1)))
+
+    def q_sample(self, x_start: torch.Tensor, t: torch.Tensor, noise: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """x_t = sqrt(abar_t) x_start + sqrt(1 - abar_t) noise.  p_losses evaluates the same inside its first kernel."""
+        noise = torch.randn_like(x_start) if noise is None else noise
+        return (self._extract(self.sqrt_alphas_cumprod, t, x_start.shape) * x_start
+                + self._extract(self.sqrt_one_minus_alphas_cumprod, t, x_start.shape) * noise)
+
+    @property
+    def loss_fn(self):
+        if self.loss_type == "l1":
+            return F.l1_loss
+        elif self.loss_type == "l2":
+            return F.mse_loss
+        raise ValueError(f"invalid loss type {self.loss_type}")
+
+    def p_losses(self, x_start: torch.Tensor, t: torch.Tensor, z: torch.Tensor = None, noise: Optional[torch.Tensor] = None):
+        """The diffusion loss of the denoiser in one native forward (q_sample, Denoiser, x_0 prediction, element-wise loss) whose
+        backward returns the 108 denoiser parameter gradients.  Dropout follows the denoiser's train()/eval() mode; its masks come
+        from one 64-bit seed drawn after the noise on the device generator."""
+        self.loss_fn  # noqa: B018 -- ValueError for an unknown loss type, as the reference raises it
+        if self.objective != "pred_noise":
+            raise NotImplementedError("objective='pred_x0' is not built: the native denoiser is trained for 'pred_noise'")
+        self._require_native()
+        if z is None:
+            raise ValueError("p_losses needs the image features z [B,N,384]")
+        noise = torch.randn_like(x_start) if noise is None else noise
+        den = self.model
+        p = den.dropout_p if den.training else 0.0
+        seed = torch.randint(0, 2**63 - 1, (1,), device=x_start.device)  # read with the timestep check: one synchronisation
+        loss, x_0_pred, x_t = den.train_step_forward(x_start, t, noise, z, p, seed, self.loss_type)
+        return {"loss": loss, "noise": noise, "x_0_pred": x_0_pred, "x_t": x_t, "t": t}
+
+    def forward(self, pose: torch.Tensor, z: torch.Tensor = None, *args, **kwargs):
+        b = len(pose)
+        t = torch.randint(0, self.num_timesteps, (b,), device=pose.device).long()
+        return self.p_losses(pose, t, z=z, *args, **kwargs)

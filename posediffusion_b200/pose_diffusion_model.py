@@ -1,5 +1,6 @@
 """`PoseDiffusionModel` facade with the reference's constructor / forward signature
-(models/pose_diffusion_model.py:35-142) for the inference branch.
+(models/pose_diffusion_model.py:35-142): the sampling branch, and the training branch (training=True) with a frozen
+image feature extractor or precomputed features.
 
 Hydra is not a dependency: the `_target_` strings of cfgs/default.yaml are resolved against this package
 (`models.Denoiser`, `models.GaussianDiffusion`, `models.TransformerEncoderWrapper`,
@@ -12,7 +13,7 @@ from typing import Dict, List, Optional
 import torch
 import torch.nn as nn
 
-from .camera_transform import pose_encoding_to_camera
+from .camera_transform import camera_to_pose_encoding, pose_encoding_to_camera
 from .denoiser import Denoiser, TransformerEncoderWrapper
 from .gaussian_diffuser import GaussianDiffusion
 from .image_feature_extractor import MultiScaleImageFeatureExtractor
@@ -58,13 +59,28 @@ class PoseDiffusionModel(nn.Module):
 
     def forward(self, image: Optional[torch.Tensor] = None, gt_cameras=None, sequence_name: Optional[List[str]] = None,
                 cond_fn=None, cond_start_step=0, training=True, batch_repeat=-1, z: Optional[torch.Tensor] = None):
-        if training:
-            raise NotImplementedError("training is outside the native sampling hot path; call with training=False")
         if z is None:
             if self.image_feature_extractor is None or image is None:
                 raise ValueError("no image feature extractor configured: pass precomputed features as z=[B,N,384]")
+            if training and any(p.requires_grad for p in self.image_feature_extractor.parameters()):
+                raise NotImplementedError(
+                    "training with a trainable image feature extractor needs the DINO ViT backward, which is not built: "
+                    "construct MultiScaleImageFeatureExtractor with freeze=True or pass precomputed features as z=")
             b, n = image.shape[:2]
             z = self.image_feature_extractor(image.reshape(b * n, *image.shape[2:])).reshape(b, n, -1)
+        if training:  # models/pose_diffusion_model.py:111-126
+            batch_num = z.shape[0]
+            pose_encoding = camera_to_pose_encoding(gt_cameras, pose_encoding_type=self.pose_encoding_type)
+            if batch_repeat > 0:
+                pose_encoding = pose_encoding.reshape(batch_num * batch_repeat, -1, self.target_dim)
+                z = z.repeat(batch_repeat, 1, 1)
+            else:
+                pose_encoding = pose_encoding.reshape(batch_num, -1, self.target_dim)
+            diffusion_results = self.diffuser(pose_encoding, z=z)
+            diffusion_results["pred_cameras"] = pose_encoding_to_camera(
+                diffusion_results["x_0_pred"].detach(), pose_encoding_type=self.pose_encoding_type
+            )
+            return diffusion_results
         B, N, _ = z.shape
         pose_encoding, _trajectory = self.diffuser.sample(
             shape=[B, N, self.target_dim], z=z, cond_fn=cond_fn, cond_start_step=cond_start_step
