@@ -236,10 +236,13 @@ int pdb_vit_load(pdb_context* ctx, const float* const* tensors, const int64_t* n
                  void* stream);
 /* interpolate_pos_encoding of the hub model for a grid_h x grid_w patch grid: bicubic resampling of the 14x14 table with the
  * scale factor (grid + 0.1) / 14 (torch F.interpolate semantics, align_corners=False).  HOST-ONLY helper, needs no GPU:
- * pos_embed_host [197,384] -> out_host [1 + grid_h*grid_w, 384]. */
+ * pos_embed_host [197,384] -> out_host [1 + grid_h*grid_w, 384].  (14, 14) means a square input and returns the stored table;
+ * the hub model resamples a 14x14 grid of a non-square image (e.g. 224x232), which pdb_extract_features does too. */
 int pdb_vit_pos_table(const float* pos_embed_host, int32_t grid_h, int32_t grid_w, float* out_host);
 /* images_dev [n,3,H,W] in [0,1] (what load_and_preprocess_images / the dataloader produce) -> z_dev [n,384].
  * scale_factors as in cfgs/default.yaml (1, 1/2, 1/3); empty -> PDB_ERR_INVALID (the reference raises ValueError, :75-76).
+ * PDB_ERR_LIMIT, before any kernel is launched, for more than 4 scales, more than 256 tokens per image at a scale, or more
+ * than 65535 images.
  * tokens_debug_dev (may be NULL): receives the residual stream [sum over scales of n*(1+gh*gw), 384] (scale-major, image, token)
  * after stage `debug_stage` (0 = prepare_tokens, k = block k) -- the parity tests' probe. */
 int pdb_extract_features(pdb_context* ctx, const float* images_dev, int32_t n_images, int32_t height, int32_t width,

@@ -29,6 +29,7 @@ constexpr int kVitPatchK = 3 * kVitPatch * kVitPatch;  // 768
 constexpr int kVitGrid0 = 14;                          // native 224 / 16 position grid
 constexpr int kVitMaxTokens = 256;                     // tokens per (image, scale) the attention kernel keeps in shared memory
 constexpr int kVitMaxScales = 4;
+constexpr int kVitMaxImages = 65535;                   // vit_patchify_kernel puts the image index on gridDim.y
 constexpr float kVitLnEps = 1e-6f;
 constexpr int kVitTensors = 4 + 12 * kVitDepth + 2;
 
@@ -396,8 +397,10 @@ __global__ void vit_head_kernel(const float* __restrict__ X, VitHeadArgs a, cons
   for (int i = 0; i < kVitDim / 32; ++i) z[(size_t)n * kVitDim + lane + 32 * i] = acc[i] / (float)a.n_scales;
 }
 
-int vit_pos_table(Context* ctx, VitWeights* w, int gh, int gw, const float** out, cudaStream_t st) {
-  if (gh == kVitGrid0 && gw == kVitGrid0) {
+// dino's interpolate_pos_encoding keeps the stored table only for 196 patches of a SQUARE image (it compares pixel sizes), so a
+// 224x232 input resamples the 14x14 grid with scale 14.1 / 14; that resampled 14x14 table is cached in pos_tables like any other.
+int vit_pos_table(Context* ctx, VitWeights* w, int gh, int gw, bool square, const float** out, cudaStream_t st) {
+  if (gh == kVitGrid0 && gw == kVitGrid0 && square) {
     *out = w->pos;
     return PDB_OK;
   }
@@ -516,6 +519,7 @@ extern "C" int pdb_extract_features(pdb_context* c, const float* images_dev, int
   if (!images_dev || !z_dev || !scale_factors) return ctx->fail(PDB_ERR_INVALID, "null argument");
   if (!ctx->vit) return ctx->fail(PDB_ERR_STATE, "image backbone weights not loaded (pdb_vit_load)");
   if (n_images < 1 || height < 1 || width < 1) return ctx->fail(PDB_ERR_INVALID, "bad image batch [%d,3,%d,%d]", n_images, height, width);
+  if (n_images > kVitMaxImages) return ctx->fail(PDB_ERR_LIMIT, "%d images in one call (limit %d)", n_images, kVitMaxImages);
   if (n_scales < 1) return ctx->fail(PDB_ERR_INVALID, "scale_factors must not be empty");  // image_feature_extractor.py:75-76 (ValueError)
   if (n_scales > kVitMaxScales) return ctx->fail(PDB_ERR_LIMIT, "at most %d scale factors", kVitMaxScales);
   PDB_CUDA(ctx, cudaSetDevice(ctx->device));
@@ -542,7 +546,7 @@ extern "C" int pdb_extract_features(pdb_context* c, const float* images_dev, int
       return ctx->fail(PDB_ERR_LIMIT, "%d tokens per image at scale %g (limit %d)", v.tokens, f, kVitMaxTokens);
     v.row0 = (int)rows;
     rows += (long long)n_images * v.tokens;
-    if (int rc = vit_pos_table(ctx, w, v.gh, v.gw, &v.pos, st)) return rc;
+    if (int rc = vit_pos_table(ctx, w, v.gh, v.gw, v.out_h == v.out_w, &v.pos, st)) return rc;
     head.row0[s] = v.row0;
     head.tokens[s] = v.tokens;
   }
@@ -618,6 +622,7 @@ extern "C" int pdb_extract_features_host(pdb_context* c, const float* images_hos
   Context* ctx = reinterpret_cast<Context*>(c);
   if (!images_host || !z_host) return ctx->fail(PDB_ERR_INVALID, "null argument");
   if (n_images < 1 || height < 1 || width < 1) return ctx->fail(PDB_ERR_INVALID, "bad image batch [%d,3,%d,%d]", n_images, height, width);
+  if (n_images > kVitMaxImages) return ctx->fail(PDB_ERR_LIMIT, "%d images in one call (limit %d)", n_images, kVitMaxImages);
   PDB_CUDA(ctx, cudaSetDevice(ctx->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t img_bytes = sizeof(float) * (size_t)n_images * 3 * height * width, z_bytes = sizeof(float) * (size_t)n_images * kVitDim;
