@@ -20,7 +20,7 @@ struct GgsBatch {
   GgsProblem prob[kGgsBatchMax];
 };
 
-template <bool kEval, bool kPaired, bool kProbe = false>
+template <bool kEval, bool kPaired, bool kProbe = false, bool kLean = false>
 __global__ void __launch_bounds__(kGgsThreads, 1)
 ggs_entry(const __grid_constant__ GgsBatch batch, const __grid_constant__ GgsParams P);
 
@@ -286,6 +286,7 @@ int finish_pack(Context* ctx, std::vector<int4>& segs, long long rounds, int64_t
   }
   m->pts = static_cast<float4*>(dpts);
   m->segs = static_cast<int4*>(dsegs);
+  m->host_segs = segs;
   cudaError_t err = cudaMemcpyAsync(m->pts, hpts, pts_bytes, cudaMemcpyHostToDevice, st);
   if (err == cudaSuccess) err = cudaMemcpyAsync(m->segs, hsegs, segs_bytes, cudaMemcpyHostToDevice, st);
   if (err == cudaSuccess) err = cudaStreamSynchronize(st);  // the staging buffer is reused by the next call
@@ -453,17 +454,18 @@ int pdb_debug_pack_layout(const double* kp1, const double* kp2, const int64_t* i
 // GGS launch plumbing (shared with the sampler in api_sampler.cu)
 // ------------------------------------------------------------------------------------------------
 namespace {
-template <bool kEval, bool kPaired, bool kProbe>
+template <bool kEval, bool kPaired, bool kProbe, bool kLean>
 __global__ void __launch_bounds__(kGgsThreads, 1)
 ggs_entry(const __grid_constant__ GgsBatch batch, const __grid_constant__ GgsParams P) {
-  ggs_body<kEval, kPaired, kProbe>(batch.prob[blockIdx.x / P.ctas_per_problem], P);
+  ggs_body<kEval, kPaired, kProbe, kLean>(batch.prob[blockIdx.x / P.ctas_per_problem], P);
 }
 
+// segs_fit: every CTA of every sequence in the batch touches at most kGgsMaxSeg segments (ggs_lean_fits)
 template <bool kEval, bool kPaired, bool kProbe = false>
 int launch_ggs_chunk(Context* ctx, const GgsBatch& batch, int nprob, int max_frames, long long max_rounds,
-                     GgsParams P, cudaStream_t st) {
+                     GgsParams P, bool segs_fit, cudaStream_t st) {
   if constexpr (!kEval && !kProbe) {  // the timing probe is its own instantiation (armed by pdb_debug_ggs_clocks, single-sequence calls)
-    if (batch.prob[0].dbg_clock) return launch_ggs_chunk<kEval, kPaired, true>(ctx, batch, nprob, max_frames, max_rounds, P, st);
+    if (batch.prob[0].dbg_clock) return launch_ggs_chunk<kEval, kPaired, true>(ctx, batch, nprob, max_frames, max_rounds, P, segs_fit, st);
   }
   const int cpp = P.ctas_per_problem;  // ggs_plan
   // shared-memory match cache: everything beyond the fixed per-frame state, in rounds of 512 B
@@ -475,10 +477,14 @@ int launch_ggs_chunk(Context* ctx, const GgsBatch& batch, int nprob, int max_fra
   const bool resident = (size_t)rounds_per_cta * 512 <= budget && !(force_stream && force_stream[0] == '1');
   P.resident_rounds = resident ? (int)rounds_per_cta : 0;
   P.ring = resident ? 0 : 1;
+  // the lean instantiation serves the case it was specialised for; PDB_GGS_LEAN=0 keeps the general kernel (tests compare the two)
+  const char* lean_env = getenv("PDB_GGS_LEAN");
+  const bool lean = !kEval && resident && segs_fit && P.xch_mode == 1 && !(lean_env && lean_env[0] == '0');
+  const void* kernel = lean ? (const void*)ggs_entry<kEval, kPaired, kProbe, !kEval> : (const void*)ggs_entry<kEval, kPaired, kProbe, false>;
   const size_t smem = fixed + (resident ? (size_t)rounds_per_cta * 512 : (size_t)kRingBytes);
-  size_t& attr_bytes = ctx->attr_ggs[(kEval ? 1 : 0) + (kPaired ? 2 : 0) + (kProbe ? 4 : 0)];
+  size_t& attr_bytes = ctx->attr_ggs[(kEval ? 1 : 0) + (kPaired ? 2 : 0) + (kProbe ? 4 : 0) + (lean ? 8 : 0)];
   if (smem > attr_bytes) {
-    PDB_CUDA(ctx, (cudaFuncSetAttribute(ggs_entry<kEval, kPaired, kProbe>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)));
+    PDB_CUDA(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_bytes = smem;
   }
   cudaLaunchConfig_t cfg = {};
@@ -493,7 +499,8 @@ int launch_ggs_chunk(Context* ctx, const GgsBatch& batch, int nprob, int max_fra
   cfg.numAttrs = 1;
   {
     ScopedTimer timer(ctx, st, 0);
-    PDB_CUDA(ctx, (cudaLaunchKernelEx(&cfg, ggs_entry<kEval, kPaired, kProbe>, batch, P)));
+    void* args[] = {const_cast<GgsBatch*>(&batch), &P};
+    PDB_CUDA(ctx, cudaLaunchKernelExC(&cfg, kernel, args));
   }
   ctx->launches += 1;
   return PDB_OK;
@@ -502,9 +509,9 @@ int launch_ggs_chunk(Context* ctx, const GgsBatch& batch, int nprob, int max_fra
 // All match sets of one launch share a stream layout (it is a property of the context they were packed on).
 template <bool kEval>
 int launch_ggs_layout(Context* ctx, int layout, const GgsBatch& batch, int nprob, int max_frames, long long max_rounds,
-                      const GgsParams& P, cudaStream_t st) {
-  if (layout == kLayoutPaired) return launch_ggs_chunk<kEval, true>(ctx, batch, nprob, max_frames, max_rounds, P, st);
-  return launch_ggs_chunk<kEval, false>(ctx, batch, nprob, max_frames, max_rounds, P, st);
+                      const GgsParams& P, bool segs_fit, cudaStream_t st) {
+  if (layout == kLayoutPaired) return launch_ggs_chunk<kEval, true>(ctx, batch, nprob, max_frames, max_rounds, P, segs_fit, st);
+  return launch_ggs_chunk<kEval, false>(ctx, batch, nprob, max_frames, max_rounds, P, segs_fit, st);
 }
 }  // namespace
 
@@ -578,8 +585,10 @@ int enqueue_ggs(Context* ctx, pdb_matches* const* problems, int batch, int frame
     }
     ggs_plan(ctx, nb, max_rounds, &P.ctas_per_problem, &P.xch_group);
     P.xch_mode = ggs_xch_mode();
+    bool segs_fit = true;
     for (int i = 0; i < nb; ++i) {
       const Matches* m = reinterpret_cast<const Matches*>(problems[b0 + i]);
+      segs_fit = segs_fit && ggs_lean_fits(m->host_segs.data(), m->nseg, m->rounds, P.ctas_per_problem, m->layout == kLayoutPaired);
       GgsProblem& p = gb.prob[i];
       p.pts = m->pts;
       p.segs = m->segs;
@@ -598,7 +607,7 @@ int enqueue_ggs(Context* ctx, pdb_matches* const* problems, int batch, int frame
       ws += ggs_ws_per_problem(max_frames, P.ctas_per_problem, P.xch_group);
     }
     const int layout = reinterpret_cast<const Matches*>(problems[b0])->layout;
-    if (int rc = launch_ggs_layout<false>(ctx, layout, gb, nb, max_frames, max_rounds, P, st)) return rc;
+    if (int rc = launch_ggs_layout<false>(ctx, layout, gb, nb, max_frames, max_rounds, P, segs_fit, st)) return rc;
   }
   return PDB_OK;
 }
@@ -658,7 +667,7 @@ int pdb_sampson_eval(pdb_context* c, const pdb_matches* pm, const float* pose_de
   p.dbg_scalars = scalars_dev;
   p.dbg_F = F_dev;
   p.dbg_G = G_dev;
-  return launch_ggs_layout<true>(ctx, m->layout, gb, 1, m->frames, m->rounds > 0 ? m->rounds : 1, P, st);
+  return launch_ggs_layout<true>(ctx, m->layout, gb, 1, m->frames, m->rounds > 0 ? m->rounds : 1, P, false, st);
 }
 
 }  // extern "C"

@@ -46,7 +46,7 @@ struct Context {
   cudaStream_t pack_stream = nullptr;  // match uploads of pdb_sample_loop_host_matches (overlap the unguided prefix)
   int tc_graph_nodes = 0;
   // cudaFuncSetAttribute is per device: remember per context (= per device) what was already requested
-  size_t attr_ggs[8] = {0, 0, 0, 0, 0, 0, 0, 0}, attr_den[16] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0}, attr_att = 0;
+  size_t attr_ggs[16] = {}, attr_den[16] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0}, attr_att = 0;
   bool attr_tc = false, attr_tc128 = false, attr_tc_deep = false;
   bool tc_pdl = true;  // programmatic dependent launch between the kernels of the tensor-core engine's step graph (PDB_TC_PDL=0: off)
   bool tc_swap = false;     // swap-AB tensor-core tiles for <= 96 tokens (pdb_debug_tc_swap); default off
@@ -93,6 +93,7 @@ struct Matches {
   size_t pts_bytes = 0, segs_bytes = 0;
   float4* pts = nullptr;   // [rounds*32]
   int4* segs = nullptr;    // [nseg+1]
+  std::vector<int4> host_segs;  // host copy of segs (the launch checks per-CTA segment counts against it: ggs_lean_fits)
   int nseg = 0;
   int rounds = 0;
   int layout = 0;          // kLayoutPlain / kLayoutPaired (ggs_layout.cuh)

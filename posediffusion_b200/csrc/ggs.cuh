@@ -144,8 +144,63 @@ __device__ __forceinline__ void sampson_match2_unit(const float4 X, const float4
 
 // All-reduce of one CTA's partial gradient vector over the `cpp` CTAs of its sequence (see the file header).  Word layout:
 // [0, 7N) gT | gq per frame, then g_fx', g_fy', clamp_sum, valid error sum (eval mode), valid count (int32).  On return
-// s_gsum holds the sums -- the same bits in every CTA -- once the caller has passed a block barrier.  Kept out of line: its
-// 16-loads-in-flight polling loops would otherwise compete for registers with the streaming loop of stage 1.
+// s_gsum holds the sums -- the same bits in every CTA -- once the caller has passed a block barrier.
+//
+// ONE hop (accumulators `accbase`): a CTA adds {value, 1} to the accumulators of the frames its segments touch (s_mine; zeros
+// if the gradient of a touched frame happens to vanish) and to the five scalars; an accumulator of frame n expects s_expect[n]
+// arrivals, a scalar `cpp`.  The valid count travels as a packed 64-bit integer {arrivals : count}.  Everybody polls until the
+// arrivals are complete.  Three buffers rotate.  On entry CTA 0 clears the buffer of iteration it-2, which is the one of it+1:
+// CTA 0 has read every slot of it-1, the scalars included, so every CTA has contributed to it-1 and finished reading it-2.
+// (A frame slot of it-1 would not do: a CTA whose segments miss that frame may still be polling it.)  The block barrier
+// orders the zeros before CTA 0's contributions to `it`, without which nobody reaches iteration it+1.
+template <bool kEval>
+__device__ __forceinline__ void ggs_exchange_acc(float* accbase, int cpp, int cta, int N, unsigned it_global, const float* s_part,
+                                                 const float* s_misc, int cta_cnt, float g_fx, float g_fy, float* s_gsum,
+                                                 const int* s_expect, const int* s_mine) {
+  const int tid = threadIdx.x;
+  const int nsum = ggs_xch_words(N);
+  if (cta == 0) {
+    float* old = accbase + (size_t)((it_global + 1u) % 3u) * nsum * kAccStride;
+    for (int e = tid; e < nsum; e += kGgsThreads) st_pair_zero(old + (size_t)e * kAccStride);
+    fence_gpu();
+    __syncthreads();
+  }
+  float* acc = accbase + (size_t)(it_global % 3u) * nsum * kAccStride;
+  for (int e = tid; e < nsum; e += kGgsThreads) {
+    float* slot = acc + (size_t)e * kAccStride;
+    if (e < N * 7) {
+      if (s_mine[e / 7]) red_pair_add(slot, s_part[e]);
+    } else if (e == N * 7 + 0) red_pair_add(slot, g_fx);
+    else if (e == N * 7 + 1) red_pair_add(slot, g_fy);
+    else if (e == N * 7 + 2) red_pair_add(slot, s_misc[4]);
+    else if (e == N * 7 + 3) red_pair_add(slot, kEval ? s_misc[5] : 0.f);
+    else red_add_u64(reinterpret_cast<unsigned long long*>(slot), (1ull << 32) | (unsigned long long)(unsigned)cta_cnt);
+  }
+  for (int e = tid; e < nsum; e += kGgsThreads) {
+    const float* slot = acc + (size_t)e * kAccStride;
+    if (e < nsum - 1) {
+      const float want = (float)(e < N * 7 ? s_expect[e / 7] : cpp);
+      float2 v;
+      for (;;) {
+        v = ld_pair(slot);
+        if (v.y == want) break;
+        ll_backoff();
+      }
+      s_gsum[e] = v.x;
+    } else {
+      unsigned long long w;
+      for (;;) {
+        w = ld_ll(reinterpret_cast<const unsigned long long*>(slot));
+        if ((unsigned)(w >> 32) == (unsigned)cpp) break;
+        ll_backoff();
+      }
+      s_gsum[e] = __uint_as_float((unsigned)w);
+    }
+  }
+}
+
+// Either exchange mode: one hop when `accbase` is set, else the flag-carrying slots.  Kept out of line: its 16-loads-in-flight
+// polling loops would otherwise compete for registers with the streaming loop of stage 1.
 template <bool kEval>
 __device__ __noinline__ void ggs_exchange(unsigned long long* xch1, unsigned long long* xch2, float* accbase, int cpp, int cta, int group,
                                           int N, unsigned it_global, const float* s_part, const float* s_misc, int cta_cnt, float g_fx,
@@ -153,47 +208,7 @@ __device__ __noinline__ void ggs_exchange(unsigned long long* xch1, unsigned lon
   const int tid = threadIdx.x;
   const int nsum = ggs_xch_words(N);
   if (accbase) {
-    // ONE hop: a CTA adds {value, 1} to the accumulators of the frames its segments touch (s_mine; zeros if the gradient of a
-    // touched frame happens to vanish) and to the five scalars; an accumulator of frame n expects s_expect[n] arrivals, a scalar
-    // `cpp`.  The valid count travels as a packed 64-bit integer {arrivals : count}.  Everybody polls until the arrivals are complete.  Three buffers rotate; CTA 0 clears the one used by the previous iteration -- every CTA
-    // has read it (they all contributed to this iteration afterwards) and nobody adds to it before two more exchanges.
-    float* acc = accbase + (size_t)(it_global % 3u) * nsum * kAccStride;
-    for (int e = tid; e < nsum; e += kGgsThreads) {
-      float* slot = acc + (size_t)e * kAccStride;
-      if (e < N * 7) {
-        if (s_mine[e / 7]) red_pair_add(slot, s_part[e]);
-      } else if (e == N * 7 + 0) red_pair_add(slot, g_fx);
-      else if (e == N * 7 + 1) red_pair_add(slot, g_fy);
-      else if (e == N * 7 + 2) red_pair_add(slot, s_misc[4]);
-      else if (e == N * 7 + 3) red_pair_add(slot, kEval ? s_misc[5] : 0.f);
-      else red_add_u64(reinterpret_cast<unsigned long long*>(slot), (1ull << 32) | (unsigned long long)(unsigned)cta_cnt);
-    }
-    for (int e = tid; e < nsum; e += kGgsThreads) {
-      const float* slot = acc + (size_t)e * kAccStride;
-      if (e < nsum - 1) {
-        const float want = (float)(e < N * 7 ? s_expect[e / 7] : cpp);
-        float2 v;
-        for (;;) {
-          v = ld_pair(slot);
-          if (v.y == want) break;
-          ll_backoff();
-        }
-        s_gsum[e] = v.x;
-      } else {
-        unsigned long long w;
-        for (;;) {
-          w = ld_ll(reinterpret_cast<const unsigned long long*>(slot));
-          if ((unsigned)(w >> 32) == (unsigned)cpp) break;
-          ll_backoff();
-        }
-        s_gsum[e] = __uint_as_float((unsigned)w);
-      }
-    }
-    if (cta == 0) {
-      float* old = accbase + (size_t)((it_global + 2u) % 3u) * nsum * kAccStride;
-      for (int e = tid; e < nsum; e += kGgsThreads) st_pair_zero(old + (size_t)e * kAccStride);
-      fence_gpu();  // the zeros are in place before this CTA's next contribution can be observed
-    }
+    ggs_exchange_acc<kEval>(accbase, cpp, cta, N, it_global, s_part, s_misc, cta_cnt, g_fx, g_fy, s_gsum, s_expect, s_mine);
     return;
   }
   const unsigned tag = it_global + 1u;
@@ -229,13 +244,36 @@ __device__ __noinline__ void ggs_exchange(unsigned long long* xch1, unsigned lon
   }
 }
 
+// Host side of the lean dispatch: true when every one of the `cpp` CTAs sharing the match set (segment descriptors `segs`,
+// sentinel included) touches at most kGgsMaxSeg pair segments, i.e. walks its slice as a single chunk.
+inline bool ggs_lean_fits(const int4* segs, int nseg, long long rounds, int cpp, bool paired) {
+  auto seg_of_round = [&](int r) {  // as in ggs_body
+    int lo = 0, hi = nseg;
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (segs[mid].x <= r) lo = mid; else hi = mid;
+    }
+    return lo;
+  };
+  for (int c = 0; c < cpp; ++c) {
+    int a0, a1;
+    ggs_cta_range(rounds, c, cpp, paired, &a0, &a1);
+    if (a1 > a0 && seg_of_round(a1 - 1) - seg_of_round(a0) + 1 > kGgsMaxSeg) return false;
+  }
+  return true;
+}
+
 // One CTA of the group that owns one sequence.  See the file header for the stage structure.
 // `resident_rounds` > 0: the CTA's whole slice of matches (<= resident_rounds rounds) is staged in shared memory
 // once per launch and every inner iteration streams it from there (no L2/HBM traffic inside the loop).
 // kProbe: the stage timing probe (tools/ggs_stage_probe.py) is a separate instantiation, so that the production kernels carry no
 // clock reads: the code one iteration executes is close to the capacity of the instruction cache.
-template <bool kEval, bool kPaired = false, bool kProbe = false>
+// kLean: the instantiation of the common case (config 3): resident slice, at most kGgsMaxSeg segments per CTA, one-hop
+// exchange, optimisation.  The host picks it only when all of that holds (ggs_lean_fits); the ring, register-stream and
+// multi-chunk stage-1 paths and the slot exchange are compiled out, which keeps the kernel free of spills and its loop small.
+template <bool kEval, bool kPaired = false, bool kProbe = false, bool kLean = false>
 __device__ __forceinline__ void ggs_body(const GgsProblem& pr, const GgsParams& P) {
+  static_assert(!(kLean && kEval), "the lean instantiation is optimisation only");
 #ifdef PDB_EMU  // tests/host/cuda_emu.h (CPU emulation of this kernel, test harness only): dynamic shared memory of this CTA
   unsigned char* const smem_raw = emu::g_cta->smem;
 #else
@@ -285,8 +323,8 @@ __device__ __forceinline__ void ggs_body(const GgsProblem& pr, const GgsParams& 
   const int seg_hi = cta_has_work ? seg_of_round(r_cta1 - 1) : -1;  // inclusive
   ggs_warp_range_seg(pr.segs, seg_lo, seg_hi, r_cta0, r_cta1, warp, kGgsWarps, kPaired, &r_w0, &r_w1);  // no warp crosses a segment
   const int wseg0 = (r_w1 > r_w0) ? seg_of_round(r_w0) : 0;
-  const bool single_chunk = (seg_hi - seg_lo + 1) <= kGgsMaxSeg;
-  const bool resident = (r_cta1 - r_cta0) <= P.resident_rounds;
+  const bool single_chunk = kLean || (seg_hi - seg_lo + 1) <= kGgsMaxSeg;
+  const bool resident = kLean || (r_cta1 - r_cta0) <= P.resident_rounds;
   const bool use_ring = !resident && single_chunk && P.ring;
   // bulk-async ring of this warp: kRingStages chunks of kGgsUnroll rounds + one mbarrier per stage
   const uint32_t ring_base = smem_u32(s_pts) + warp * (kRingStages * kGgsUnroll * 512);
@@ -413,7 +451,7 @@ __device__ __forceinline__ void ggs_body(const GgsProblem& pr, const GgsParams& 
       if (kProbe && pr.dbg_clock && tid == 0) ck0 = clock64();
       // ================= chunks of <= kGgsMaxSeg pair segments (one chunk in all practical cases) =================
       for (int cs = seg_lo; cs <= seg_hi; cs += kGgsMaxSeg) {
-        const int ce = min(cs + kGgsMaxSeg, seg_hi + 1);
+        const int ce = kLean ? seg_hi + 1 : min(cs + kGgsMaxSeg, seg_hi + 1);
         const int nchunk = ce - cs;
         if (!single_chunk) {
           __syncthreads();
@@ -699,6 +737,7 @@ __device__ __forceinline__ void ggs_body(const GgsProblem& pr, const GgsParams& 
             atomicAdd(&s_misc[5], gs);
           }
         }
+        if (kLean) break;  // one chunk
       }
       __syncthreads();
       if (kProbe && pr.dbg_clock && tid == 0) ck1 = clock64();
@@ -736,8 +775,13 @@ __device__ __forceinline__ void ggs_body(const GgsProblem& pr, const GgsParams& 
       __syncthreads();
       if (kProbe && pr.dbg_clock && tid == 0) ck2 = clock64();
       // ================= exchange: all-reduce of the partial gradient over the CTAs of this sequence =================
-      ggs_exchange<kEval>(pr.xch1, pr.xch2, P.xch_mode == 1 ? pr.acc : nullptr, cpp, cta, P.xch_group, N, it_global, s_part, s_misc, s_cta_cnt,
-                          (-s_misc[8] + cx * s_misc[10]) / (fpx * fpx), (-s_misc[9] + cy * s_misc[11]) / (fpy * fpy), s_gsum, s_expect, s_mine);
+      if constexpr (kLean) {
+        const float g_fx = (-s_misc[8] + cx * s_misc[10]) / (fpx * fpx), g_fy = (-s_misc[9] + cy * s_misc[11]) / (fpy * fpy);
+        ggs_exchange_acc<kEval>(pr.acc, cpp, cta, N, it_global, s_part, s_misc, s_cta_cnt, g_fx, g_fy, s_gsum, s_expect, s_mine);
+      } else {
+        ggs_exchange<kEval>(pr.xch1, pr.xch2, P.xch_mode == 1 ? pr.acc : nullptr, cpp, cta, P.xch_group, N, it_global, s_part, s_misc, s_cta_cnt,
+                            (-s_misc[8] + cx * s_misc[10]) / (fpx * fpx), (-s_misc[9] + cy * s_misc[11]) / (fpy * fpy), s_gsum, s_expect, s_mine);
+      }
       ++it_global;
       __syncthreads();
       if (kProbe && pr.dbg_clock && tid == 0) {
