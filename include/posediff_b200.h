@@ -306,12 +306,32 @@ int pdb_train_forward(pdb_context* ctx, const float* const* params, const float*
  * timestep flag).  Bit-reproducible: no floating-point atomics. */
 int pdb_train_backward(pdb_context* ctx, const float* const* params, void* workspace, const float* grad_loss_dev, const float* grad_x0_dev,
                        float* const* grads, void* stream);
+/* pdb_train_backward that also writes grad_z_dev [B,N,384] = d(...) / d z (NULL: exactly pdb_train_backward).  The 108 parameter
+ * gradients do not depend on whether grad_z_dev is given. */
+int pdb_train_backward_z(pdb_context* ctx, const float* const* params, void* workspace, const float* grad_loss_dev, const float* grad_x0_dev,
+                         float* const* grads, float* grad_z_dev, void* stream);
 /* camera_to_pose_encoding, "absT_quaR_logFL" (util/camera_transform.py:108-129): R [count,3,3], T [count,3], focal [count,2] ->
  * pose [count,9] = T | matrix_to_quaternion(R) with the real part made non-negative | log(clamp(focal, min, max)) - bias. */
 int pdb_camera_to_pose(pdb_context* ctx, const float* R_dev, const float* T_dev, const float* focal_dev, int32_t count,
                        double log_focal_length_bias, double min_focal_length, double max_focal_length, float* pose_dev, void* stream);
 /* HOST-ONLY: out[i] = 1 if element offset + i of (layer, site) is kept under the dropout rule above, else 0. */
 int pdb_dropout_mask_host(uint64_t seed, int32_t layer, int32_t site, int64_t offset, int64_t count, float dropout_p, uint8_t* out);
+
+/* ---- training the image backbone (MultiScaleImageFeatureExtractor with freeze=False) --------------------------------------------
+ * tensors[150] are the DINO ViT-S/16 parameters in pdb_vit_load order, device fp32, contiguous, 16-byte aligned, read where they
+ * are on every call (pdb_vit_load is not needed and its copy is not used).  LayerNorm is applied explicitly (not folded into the
+ * qkv / fc1 weights as pdb_extract_features does), so z differs from pdb_extract_features' z by the folding's rounding.
+ * The workspace (device, 16-byte aligned, pdb_vit_train_workspace_bytes) is owned by the caller: the forward saves the activations
+ * the backward needs in it, the backward also uses it as scratch.  Same shape limits as pdb_extract_features. */
+int64_t pdb_vit_train_workspace_bytes(int32_t n_images, int32_t height, int32_t width, const double* scale_factors,
+                                      int32_t n_scales); /* 0 for an unsupported shape */
+/* images_dev [n,3,H,W] in [0,1] -> z_dev [n,384].  Synchronises the stream once per resampled scale (position-table taps upload). */
+int pdb_vit_train_forward(pdb_context* ctx, const float* const* tensors, const float* images_dev, int32_t n_images, int32_t height,
+                          int32_t width, const double* scale_factors, int32_t n_scales, void* workspace, float* z_dev, void* stream);
+/* grads[150] (device, parameter shapes) are overwritten with d(sum(grad_z * z)) / d tensors; there is no gradient to the images.
+ * Synchronises the stream once to read the workspace header.  Bit-reproducible: no floating-point atomics. */
+int pdb_vit_backward(pdb_context* ctx, const float* const* tensors, void* workspace, const float* grad_z_dev, float* const* grads,
+                     void* stream);
 
 #ifdef __cplusplus
 }

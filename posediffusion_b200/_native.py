@@ -103,6 +103,12 @@ EXPORTS = {
     "pdb_train_forward": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                     C.c_float, C.c_uint64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pdb_train_backward": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p]),
+    "pdb_train_backward_z": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p,
+                                       C.c_void_p]),
+    "pdb_vit_train_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_double), C.c_int32]),
+    "pdb_vit_train_forward": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_double),
+                                        C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pdb_vit_backward": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p]),
     "pdb_camera_to_pose": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_double, C.c_double, C.c_double,
                                      C.c_void_p, C.c_void_p]),
     "pdb_dropout_mask_host": (C.c_int, [C.c_uint64, C.c_int32, C.c_int32, C.c_int64, C.c_int64, C.c_float, C.c_void_p]),
@@ -126,6 +132,13 @@ def dropout_mask_host(seed: int, layer: int, site: int, offset: int, count: int,
 
 def train_workspace_bytes(batch: int, frames: int) -> int:
     return int(load_library().pdb_train_workspace_bytes(int(batch), int(frames)))
+
+
+def vit_train_workspace_bytes(n_images: int, height: int, width: int, scale_factors: Sequence[float]) -> int:
+    """Bytes of the workspace a backbone training forward of this shape needs; 0 for an unsupported shape (no GPU needed)."""
+    sf = (C.c_double * max(len(scale_factors), 1))(*[float(f) for f in scale_factors])
+    return int(load_library().pdb_vit_train_workspace_bytes(int(n_images), int(height), int(width), sf, len(scale_factors)))
+
 
 _lib = None
 _lib_lock = threading.Lock()
@@ -379,15 +392,21 @@ class Context:
         return ws, loss, x_t, x0
 
     def train_backward(self, params: Sequence[torch.Tensor], ws: torch.Tensor, grad_loss: Optional[torch.Tensor],
-                       grad_x0: Optional[torch.Tensor]) -> List[torch.Tensor]:
+                       grad_x0: Optional[torch.Tensor], grad_z: Optional[torch.Tensor] = None) -> List[torch.Tensor]:
+        """Gradients of the 108 parameters; with `grad_z` (a [B,N,384] buffer) also dL/dz, written into it."""
         arr = self._param_array(params)
         grads = [torch.empty_like(p) for p in params]
         garr = (C.c_void_p * len(grads))(*[C.c_void_p(g.data_ptr()) for g in grads])
+        gl = grad_loss.data_ptr() if grad_loss is not None else None
+        gx = grad_x0.data_ptr() if grad_x0 is not None else None
         with torch.cuda.device(self.device):
-            self._ok(self.lib.pdb_train_backward(self.handle, arr, ws.data_ptr(),
-                                                 grad_loss.data_ptr() if grad_loss is not None else None,
-                                                 grad_x0.data_ptr() if grad_x0 is not None else None, garr, _stream_ptr(self.device)),
-                     "pdb_train_backward")
+            if grad_z is None:
+                self._ok(self.lib.pdb_train_backward(self.handle, arr, ws.data_ptr(), gl, gx, garr, _stream_ptr(self.device)),
+                         "pdb_train_backward")
+            else:
+                _check_dev(grad_z, "grad_z", self.device)
+                self._ok(self.lib.pdb_train_backward_z(self.handle, arr, ws.data_ptr(), gl, gx, garr, grad_z.data_ptr(),
+                                                       _stream_ptr(self.device)), "pdb_train_backward_z")
         return grads
 
     def camera_to_pose(self, R: torch.Tensor, T: torch.Tensor, focal: torch.Tensor, log_focal_length_bias=1.8, min_focal_length=0.1,
@@ -492,6 +511,47 @@ class Context:
                                                    C.c_void_p(z.data_ptr()), C.c_void_p(dbg.data_ptr()) if dbg is not None else None,
                                                    int(debug_stage or 0), _stream_ptr(self.device)), "pdb_extract_features")
         return (z, dbg) if debug_stage is not None else z
+
+    # ---- backbone training ----------------------------------------------------------------------------
+    def _vit_array(self, tensors: Sequence[torch.Tensor], what: str):
+        if len(tensors) != PDB_VIT_NUM_TENSORS:
+            raise NativeError(f"expected {PDB_VIT_NUM_TENSORS} tensors, got {len(tensors)}")
+        for i, p in enumerate(tensors):
+            _check_dev(p, f"{what} {i}", self.device)
+        return (C.c_void_p * len(tensors))(*[C.c_void_p(p.data_ptr()) for p in tensors])
+
+    def vit_train_workspace_bytes(self, n_images: int, height: int, width: int, scale_factors: Sequence[float]) -> int:
+        return vit_train_workspace_bytes(n_images, height, width, scale_factors)
+
+    def vit_train_forward(self, params: Sequence[torch.Tensor], images: torch.Tensor, scale_factors: Sequence[float]):
+        """Backbone forward that keeps what vit_backward needs: returns (workspace, z [n,384]).  The workspace belongs to the
+        caller (one per outstanding forward).  `params`: the 150 tensors in hub state_dict order, on this device."""
+        n, ch, H, W = images.shape
+        if ch != 3:
+            raise NativeError(f"images must be [n,3,H,W], got {tuple(images.shape)}")
+        _check_dev(images, "images", self.device)
+        nbytes = vit_train_workspace_bytes(n, H, W, scale_factors)
+        if nbytes <= 0:
+            raise NativeError(f"unsupported backbone training shape: {n} images of {H}x{W} at scales {list(scale_factors)}")
+        arr = self._vit_array(params, "parameter")
+        sf = (C.c_double * len(scale_factors))(*[float(f) for f in scale_factors])
+        ws = torch.empty(nbytes // 4, dtype=torch.float32, device=self.device)
+        z = torch.empty((n, VIT_DIM), device=self.device, dtype=torch.float32)
+        with torch.cuda.device(self.device):
+            self._ok(self.lib.pdb_vit_train_forward(self.handle, arr, images.data_ptr(), n, H, W, sf, len(scale_factors), ws.data_ptr(),
+                                                    z.data_ptr(), _stream_ptr(self.device)), "pdb_vit_train_forward")
+        return ws, z
+
+    def vit_backward(self, params: Sequence[torch.Tensor], ws: torch.Tensor, grad_z: torch.Tensor) -> List[torch.Tensor]:
+        """d(sum(grad_z * z)) / d params for the forward held in `ws`."""
+        arr = self._vit_array(params, "parameter")
+        _check_dev(grad_z, "grad_z", self.device)
+        grads = [torch.empty_like(p) for p in params]
+        garr = (C.c_void_p * len(grads))(*[C.c_void_p(g.data_ptr()) for g in grads])
+        with torch.cuda.device(self.device):
+            self._ok(self.lib.pdb_vit_backward(self.handle, arr, ws.data_ptr(), grad_z.data_ptr(), garr, _stream_ptr(self.device)),
+                     "pdb_vit_backward")
+        return grads
 
     def extract_features_host(self, images: np.ndarray, scale_factors: Sequence[float]) -> np.ndarray:
         n, ch, H, W = images.shape

@@ -17,7 +17,7 @@ ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 OBJ = os.path.join(ROOT, "build", "obj")
 LIB = os.path.join(PKG, "libposediff_b200.so")
-SOURCES = ["api_core.cu", "api_sampler.cu", "api_tc.cu", "api_vit.cu", "api_post.cu", "api_pre.cu", "api_train.cu"]
+SOURCES = ["api_core.cu", "api_sampler.cu", "api_tc.cu", "api_vit.cu", "api_post.cu", "api_pre.cu", "api_train.cu", "api_vit_train.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xptxas", "-v", f"-I{os.path.join(ROOT, 'include')}", f"-I{CSRC}"]
 

@@ -176,12 +176,12 @@ extern "C" int pdb_train_forward(pdb_context* c, const float* const* params, con
   const long long nd = (long long)S * kDM, nf = (long long)S * kFF;
   for (int l = 0; l < kLayers; ++l) {
     const int b = 6 + 12 * l;
-    train_ln_fwd_kernel<kDM><<<blocks(S, 8), 256, 0, st>>>(ws + L.hin[l], W(b + 8), W(b + 9), S, ws + L.a1[l], ws + L.st1[l]);
+    train_ln_fwd_kernel<kDM><<<blocks(S, 8), 256, 0, st>>>(ws + L.hin[l], W(b + 8), W(b + 9), S, kLnEps, ws + L.a1[l], ws + L.st1[l]);
     if (int rc = gemm(ctx, ws + L.a1[l], W(b + 0), W(b + 1), ws + L.qkv[l], S, 3 * kDM, kDM, 0, st)) return rc;
     train_attn_fwd_kernel<<<B * kHeads, 256, attn_fwd_smem(N), st>>>(ws + L.qkv[l], N, d, l, ws + L.P[l], ws + L.att[l]);
     if (int rc = gemm(ctx, ws + L.att[l], W(b + 2), W(b + 3), ws + L.G1, S, kDM, kDM, 0, st)) return rc;
     train_dropout_kernel<<<blocks(nd), 256, 0, st>>>(ws + L.G1, ws + L.hin[l], nullptr, ws + L.hmid[l], nd, d, l, kSiteOut);
-    train_ln_fwd_kernel<kDM><<<blocks(S, 8), 256, 0, st>>>(ws + L.hmid[l], W(b + 10), W(b + 11), S, ws + L.a2[l], ws + L.st2[l]);
+    train_ln_fwd_kernel<kDM><<<blocks(S, 8), 256, 0, st>>>(ws + L.hmid[l], W(b + 10), W(b + 11), S, kLnEps, ws + L.a2[l], ws + L.st2[l]);
     if (int rc = gemm(ctx, ws + L.a2[l], W(b + 4), W(b + 5), ws + L.fd[l], S, kFF, kDM, 1, st)) return rc;
     train_dropout_kernel<<<blocks(nf), 256, 0, st>>>(ws + L.fd[l], nullptr, nullptr, ws + L.fd[l], nf, d, l, kSiteRelu);
     if (int rc = gemm(ctx, ws + L.fd[l], W(b + 6), W(b + 7), ws + L.G1, S, kDM, kFF, 0, st)) return rc;
@@ -198,10 +198,16 @@ extern "C" int pdb_train_forward(pdb_context* c, const float* const* params, con
 
 extern "C" int pdb_train_backward(pdb_context* c, const float* const* params, void* workspace, const float* grad_loss, const float* grad_x0,
                                   float* const* grads, void* stream) {
+  return pdb_train_backward_z(c, params, workspace, grad_loss, grad_x0, grads, nullptr, stream);
+}
+
+extern "C" int pdb_train_backward_z(pdb_context* c, const float* const* params, void* workspace, const float* grad_loss,
+                                    const float* grad_x0, float* const* grads, float* grad_z, void* stream) {
   if (!c) return PDB_ERR_INVALID;
   Context* ctx = reinterpret_cast<Context*>(c);
   if (int rc = check_params(ctx, params)) return rc;
   if (!workspace || !grads) return ctx->fail(PDB_ERR_INVALID, "null argument");
+  if (grad_z && !aligned16(grad_z)) return ctx->fail(PDB_ERR_INVALID, "grad_z is not 16-byte aligned");
   for (int i = 0; i < PDB_NUM_WEIGHT_TENSORS; ++i)
     if (!grads[i] || !aligned16(grads[i])) return ctx->fail(PDB_ERR_INVALID, "gradient %d is null or not 16-byte aligned", i);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -290,6 +296,14 @@ extern "C" int pdb_train_backward(pdb_context* c, const float* const* params, vo
   train_time_dw_kernel<<<blocks(128 * 128), 256, 0, st>>>(ws + L.dtemb, ws + L.u1, tsv, B, 128, 1, G(2), G(3));
   train_time_dw_kernel<<<blocks(128 * 256), 256, 0, st>>>(ws + L.du1, ws + L.u1, tsv, B, 256, 0, G(0), G(1));
   ctx->launches += 20 + kLayers * 40;
+  if (grad_z) {
+    // dz = dh0 . W_first[:, 317:701]: the column block starts at float 317, which TMA cannot address, so it is copied to an
+    // aligned [512, 384] buffer (the _first weight-gradient staging area, free by now) and then read K-major like every dX
+    float* Wz = ws + L.dWf;
+    train_copy_cols_kernel<<<blocks((long long)kDM * kZ), 256, 0, st>>>(W(4) + 317, kFirstIn, kDM, kZ, Wz, kZ);
+    if (int rc = input_grad(D0, Wz, kDM, kZ, grad_z)) return rc;
+    ctx->launches += 2;
+  }
   PDB_CUDA(ctx, cudaGetLastError());
   return PDB_OK;
 }

@@ -2,10 +2,13 @@
 // Projections run on the tensor-core linear layer (tc_linear.cuh); everything here is fp32 element-wise, LayerNorm,
 // attention and reduction code.  Every reduction over tokens is split into a fixed number of token chunks and the chunk
 // partials are added in chunk order: no floating-point atomics, the same inputs give bit-identical gradients.
+// The backbone's training path (csrc/api_vit_train.cu) uses the LayerNorm, transpose and column-sum kernels too; the kernels sit
+// in an anonymous namespace so that each including translation unit owns its copy.
 #pragma once
 #include <cstdint>
 
 #include "common.cuh"
+#include "posediff_b200.h"
 
 namespace pdb {
 
@@ -56,6 +59,11 @@ struct DropCfg {
 struct TrainSched {
   float c[PDB_NUM_TIMESTEPS][4];
 };
+
+}  // namespace pdb
+
+namespace {
+using namespace pdb;
 
 // ---- forward -----------------------------------------------------------------------------------------------------------------
 // time MLP per sequence: [cos(t f) | sin(t f)] -> Linear(256,128) -> SiLU -> Linear(128,128).  One block of 128 threads per sequence.
@@ -116,10 +124,10 @@ __global__ void train_feed_kernel(const __grid_constant__ TrainSched sc, const f
   }
 }
 
-// LayerNorm over C columns (eps 1e-5, biased variance), one warp per row; stats[row] = {mean, rstd}
+// LayerNorm over C columns (biased variance), one warp per row; stats[row] = {mean, rstd}
 template <int C>
 __global__ void train_ln_fwd_kernel(const float* __restrict__ x, const float* __restrict__ g, const float* __restrict__ bta, int S,
-                                    float* __restrict__ y, float* __restrict__ stats) {
+                                    float eps, float* __restrict__ y, float* __restrict__ stats) {
   constexpr int P = C / 32;
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (row >= S) return;
@@ -134,7 +142,7 @@ __global__ void train_ln_fwd_kernel(const float* __restrict__ x, const float* __
   float sq = 0.f;
 #pragma unroll
   for (int i = 0; i < P; ++i) sq += (v[i] - mean) * (v[i] - mean);
-  const float rstd = 1.0f / sqrtf(warp_sum(sq) * (1.0f / C) + 1e-5f);
+  const float rstd = 1.0f / sqrtf(warp_sum(sq) * (1.0f / C) + eps);
 #pragma unroll
   for (int i = 0; i < P; ++i) {
     const int c = lane + 32 * i;
@@ -503,4 +511,4 @@ __global__ void train_time_dw_kernel(const float* __restrict__ dy, const float* 
   if (k == 0) db[o] = bsum;
 }
 
-}  // namespace pdb
+}  // namespace

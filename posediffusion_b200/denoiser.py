@@ -51,12 +51,14 @@ class TimeStepEmbedding(nn.Module):
 
 class _DiffusionLoss(torch.autograd.Function):
     """Native p_losses: forward (pdb_train_forward) saves its activations in a workspace tensor that this graph node owns; backward
-    (pdb_train_backward) returns the gradients of the 108 parameters.  The parameters are saved for backward, so changing one in
-    place between the two raises torch's version error."""
+    (pdb_train_backward / pdb_train_backward_z) returns the gradients of the 108 parameters and, when the image features `z`
+    require grad (a trainable image feature extractor), dL/dz.  The parameters are saved for backward, so changing one in place
+    between the two raises torch's version error."""
 
     @staticmethod
-    def forward(fctx, ctx, args, dropout_p, seed, loss_type, *params):
-        ws, loss, x_t, x0 = ctx.train_forward(params, *args, dropout_p, seed, loss_type)
+    def forward(fctx, ctx, args, dropout_p, seed, loss_type, z, *params):
+        x_start, t, noise = args
+        ws, loss, x_t, x0 = ctx.train_forward(params, x_start, t, noise, z, dropout_p, seed, loss_type)
         fctx.native, fctx.ws = ctx, ws
         fctx.save_for_backward(*params)
         fctx.mark_non_differentiable(x_t)
@@ -67,10 +69,14 @@ class _DiffusionLoss(torch.autograd.Function):
         params = fctx.saved_tensors
         if fctx.ws is None:
             raise RuntimeError("the native training graph was already backpropagated and its workspace released")
+        grad_z = None
+        if fctx.needs_input_grad[5]:
+            grad_z = torch.empty(grad_loss.shape[:2] + (_native.Z_DIM,) if grad_loss is not None else grad_x0.shape[:2] + (_native.Z_DIM,),
+                                 device=params[0].device, dtype=torch.float32)
         grads = fctx.native.train_backward(params, fctx.ws, None if grad_loss is None else grad_loss.contiguous(),
-                                           None if grad_x0 is None else grad_x0.contiguous())
+                                           None if grad_x0 is None else grad_x0.contiguous(), grad_z)
         fctx.ws = None
-        return (None, None, None, None, None, *grads)
+        return (None, None, None, None, None, grad_z, *grads)
 
 
 class Denoiser(nn.Module):
@@ -126,15 +132,16 @@ class Denoiser(nn.Module):
         self._native_epoch += 1
 
     def train_step_forward(self, x_start, t, noise, z, dropout_p: float, seed, loss_type: str):
-        """(loss, x_0_pred, x_t) of GaussianDiffusion.p_losses with autograd into this module's parameters (_DiffusionLoss).
+        """(loss, x_0_pred, x_t) of GaussianDiffusion.p_losses with autograd into this module's parameters and into `z` when it
+        requires grad (_DiffusionLoss).
         `seed` is the 64-bit dropout seed, an int or a one-element integer tensor; timesteps outside [0, 100) raise IndexError."""
         params = self.ordered_parameters()
         device = params[0].device
         if device.type != "cuda":
             raise _native.NativeError("Denoiser parameters are on the CPU: call .to('cuda') (no CPU fallback)")
-        if torch.is_grad_enabled() and (x_start.requires_grad or z.requires_grad or noise.requires_grad):
-            raise NotImplementedError("gradients reach the denoiser parameters only: x_start, noise and z must not require grad "
-                                      "(train with a frozen image feature extractor)")
+        if torch.is_grad_enabled() and (x_start.requires_grad or noise.requires_grad):
+            raise NotImplementedError("gradients reach the denoiser parameters and the image features z only: x_start and noise "
+                                      "must not require grad")
         # t out of range and the seed (an int, or a one-element int64 tensor drawn on the device) in one device-to-host read
         bad = ((t < 0) | (t >= _native.NUM_TIMESTEPS)).any().view(1).to(torch.int64)
         if torch.is_tensor(seed):
@@ -144,9 +151,8 @@ class Denoiser(nn.Module):
         if bad_v:
             raise IndexError(f"timesteps must lie in [0, {_native.NUM_TIMESTEPS})")
         ctx = _native.Context.get(device)
-        args = (x_start.detach().contiguous().float(), t.to(torch.int32).contiguous(), noise.detach().contiguous().float(),
-                z.detach().contiguous().float())
-        return _DiffusionLoss.apply(ctx, args, float(dropout_p), seed_v, loss_type, *params)
+        args = (x_start.detach().contiguous().float(), t.to(torch.int32).contiguous(), noise.detach().contiguous().float())
+        return _DiffusionLoss.apply(ctx, args, float(dropout_p), seed_v, loss_type, z.contiguous().float(), *params)
 
     def forward(self, x: torch.Tensor, t: torch.Tensor, z: torch.Tensor) -> torch.Tensor:
         """x [B,N,9], t [B] (all entries equal, as the sampler passes them), z [B,N,384] -> eps [B,N,9]."""

@@ -4,6 +4,10 @@ The backbone the reference downloads with `torch.hub.load("facebookresearch/dino
 `DinoViTSmall16`, a parameter container with the hub checkpoint's names and shapes (so the released checkpoint's
 `image_feature_extractor._net.*` keys load strictly).  It has no PyTorch forward: features come from the native library
 (pdb_extract_features -- patch embedding, the 12 blocks and the head as wgmma/TMA GEMMs + shared-memory attention).
+
+With `freeze=False` (the released training recipe) and grad enabled, the forward runs the training path instead
+(pdb_vit_train_forward / pdb_vit_backward through `_BackboneFeatures`): explicit LayerNorm, activations saved in a workspace the
+autograd node owns, gradients into all 150 backbone tensors.
 """
 from __future__ import annotations
 
@@ -67,6 +71,28 @@ class DinoViTSmall16(nn.Module):
         raise RuntimeError("DinoViTSmall16 holds parameters only; call MultiScaleImageFeatureExtractor (native CUDA path)")
 
 
+class _BackboneFeatures(torch.autograd.Function):
+    """Native backbone forward whose activations live in a workspace tensor this graph node owns; backward (pdb_vit_backward)
+    returns the gradients of the 150 parameters (none for the images).  The parameters are saved for backward, so changing one
+    in place between the two raises torch's version error."""
+
+    @staticmethod
+    def forward(fctx, ctx, images, scale_factors, *params):
+        ws, z = ctx.vit_train_forward(params, images, scale_factors)
+        fctx.native, fctx.ws = ctx, ws
+        fctx.save_for_backward(*params)
+        return z
+
+    @staticmethod
+    def backward(fctx, grad_z):
+        params = fctx.saved_tensors
+        if fctx.ws is None:
+            raise RuntimeError("the native training graph was already backpropagated and its workspace released")
+        grads = fctx.native.vit_backward(params, fctx.ws, grad_z.contiguous().float())
+        fctx.ws = None
+        return (None, None, None, *grads)
+
+
 class MultiScaleImageFeatureExtractor(nn.Module):
     def __init__(self, modelname: str = "dino_vits16", freeze: bool = False, scale_factors: Sequence[float] = (1, 1 / 2, 1 / 3)):
         super().__init__()
@@ -94,12 +120,16 @@ class MultiScaleImageFeatureExtractor(nn.Module):
             ctx.load_vit(params)
             ctx.vit_key = key
 
-    @torch.no_grad()
     def forward(self, image_rgb: torch.Tensor) -> torch.Tensor:
         if len(self.scale_factors) <= 0:
             raise ValueError(f"Wrong format of self.scale_factors: {self.scale_factors}")  # :75-76
         if not image_rgb.is_cuda:
             raise _native.NativeError("image_rgb must be a CUDA tensor (posediffusion_b200 has no CPU fallback)")
         ctx = _native.Context.get(image_rgb.device)
-        self._sync_weights(ctx)
-        return ctx.extract_features(image_rgb.to(torch.float32).contiguous(), self.scale_factors)
+        images = image_rgb.detach().to(torch.float32).contiguous()
+        params = list(self._net.parameters())  # registration order = hub state_dict order (the module has no buffers)
+        if torch.is_grad_enabled() and any(p.requires_grad for p in params):
+            return _BackboneFeatures.apply(ctx, images, tuple(self.scale_factors), *params)
+        with torch.no_grad():
+            self._sync_weights(ctx)
+            return ctx.extract_features(images, self.scale_factors)

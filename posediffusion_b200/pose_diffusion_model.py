@@ -1,6 +1,6 @@
 """`PoseDiffusionModel` facade with the reference's constructor / forward signature
-(models/pose_diffusion_model.py:35-142): the sampling branch, and the training branch (training=True) with a frozen
-image feature extractor or precomputed features.
+(models/pose_diffusion_model.py:35-142): the sampling branch, and the training branch (training=True) with a frozen or a
+trainable (`freeze: False`, the released recipe) image feature extractor, or precomputed features.
 
 Hydra is not a dependency: the `_target_` strings of cfgs/default.yaml are resolved against this package
 (`models.Denoiser`, `models.GaussianDiffusion`, `models.TransformerEncoderWrapper`,
@@ -62,12 +62,17 @@ class PoseDiffusionModel(nn.Module):
         if z is None:
             if self.image_feature_extractor is None or image is None:
                 raise ValueError("no image feature extractor configured: pass precomputed features as z=[B,N,384]")
-            if training and any(p.requires_grad for p in self.image_feature_extractor.parameters()):
+            if training and not image.is_cuda and any(p.requires_grad for p in self.image_feature_extractor.parameters()):
                 raise NotImplementedError(
-                    "training with a trainable image feature extractor needs the DINO ViT backward, which is not built: "
-                    "construct MultiScaleImageFeatureExtractor with freeze=True or pass precomputed features as z=")
+                    "training with a trainable image feature extractor: the DINO ViT backward is native CUDA only, move the model "
+                    "and the images to the GPU (or construct MultiScaleImageFeatureExtractor with freeze=True, or pass z=)")
             b, n = image.shape[:2]
-            z = self.image_feature_extractor(image.reshape(b * n, *image.shape[2:])).reshape(b, n, -1)
+            flat = image.reshape(b * n, *image.shape[2:])
+            if training:
+                z = self.image_feature_extractor(flat).reshape(b, n, -1)
+            else:
+                with torch.no_grad():  # sampling: features carry no graph
+                    z = self.image_feature_extractor(flat).reshape(b, n, -1)
         if training:  # models/pose_diffusion_model.py:111-126
             batch_num = z.shape[0]
             pose_encoding = camera_to_pose_encoding(gt_cameras, pose_encoding_type=self.pose_encoding_type)
