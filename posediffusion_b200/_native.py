@@ -363,11 +363,11 @@ class Context:
             self._ok(self.lib.pdb_denoiser_load(self.handle, arr, len(keep), _stream_ptr(self.device)), "pdb_denoiser_load")
 
     # ---- training ------------------------------------------------------------------------------------
-    def _param_array(self, tensors: Sequence[torch.Tensor]):
-        if len(tensors) != PDB_NUM_WEIGHT_TENSORS:
-            raise NativeError(f"expected {PDB_NUM_WEIGHT_TENSORS} tensors, got {len(tensors)}")
+    def _tensor_array(self, tensors: Sequence[torch.Tensor], count: int, what: str):
+        if len(tensors) != count:
+            raise NativeError(f"expected {count} tensors, got {len(tensors)}")
         for i, p in enumerate(tensors):
-            _check_dev(p, f"parameter {i}", self.device)
+            _check_dev(p, f"{what} {i}", self.device)
         return (C.c_void_p * len(tensors))(*[C.c_void_p(p.data_ptr()) for p in tensors])
 
     def train_forward(self, params: Sequence[torch.Tensor], x_start, t, noise, z, dropout_p: float, seed: int, loss_type: str):
@@ -383,7 +383,7 @@ class Context:
         nbytes = train_workspace_bytes(B, N)
         ws = torch.empty(nbytes // 4, dtype=torch.float32, device=self.device)
         loss, x_t, x0 = torch.empty_like(x_start), torch.empty_like(x_start), torch.empty_like(x_start)
-        arr = self._param_array(params)
+        arr = self._tensor_array(params, PDB_NUM_WEIGHT_TENSORS, "parameter")
         with torch.cuda.device(self.device):
             self._ok(self.lib.pdb_train_forward(self.handle, arr, x_start.data_ptr(), t.data_ptr(), noise.data_ptr(), z.data_ptr(), B, N,
                                                 float(dropout_p), int(seed) & (2**64 - 1), LOSS_TYPES[loss_type], ws.data_ptr(),
@@ -394,7 +394,7 @@ class Context:
     def train_backward(self, params: Sequence[torch.Tensor], ws: torch.Tensor, grad_loss: Optional[torch.Tensor],
                        grad_x0: Optional[torch.Tensor], grad_z: Optional[torch.Tensor] = None) -> List[torch.Tensor]:
         """Gradients of the 108 parameters; with `grad_z` (a [B,N,384] buffer) also dL/dz, written into it."""
-        arr = self._param_array(params)
+        arr = self._tensor_array(params, PDB_NUM_WEIGHT_TENSORS, "parameter")
         grads = [torch.empty_like(p) for p in params]
         garr = (C.c_void_p * len(grads))(*[C.c_void_p(g.data_ptr()) for g in grads])
         gl = grad_loss.data_ptr() if grad_loss is not None else None
@@ -513,13 +513,6 @@ class Context:
         return (z, dbg) if debug_stage is not None else z
 
     # ---- backbone training ----------------------------------------------------------------------------
-    def _vit_array(self, tensors: Sequence[torch.Tensor], what: str):
-        if len(tensors) != PDB_VIT_NUM_TENSORS:
-            raise NativeError(f"expected {PDB_VIT_NUM_TENSORS} tensors, got {len(tensors)}")
-        for i, p in enumerate(tensors):
-            _check_dev(p, f"{what} {i}", self.device)
-        return (C.c_void_p * len(tensors))(*[C.c_void_p(p.data_ptr()) for p in tensors])
-
     def vit_train_workspace_bytes(self, n_images: int, height: int, width: int, scale_factors: Sequence[float]) -> int:
         return vit_train_workspace_bytes(n_images, height, width, scale_factors)
 
@@ -533,7 +526,7 @@ class Context:
         nbytes = vit_train_workspace_bytes(n, H, W, scale_factors)
         if nbytes <= 0:
             raise NativeError(f"unsupported backbone training shape: {n} images of {H}x{W} at scales {list(scale_factors)}")
-        arr = self._vit_array(params, "parameter")
+        arr = self._tensor_array(params, PDB_VIT_NUM_TENSORS, "parameter")
         sf = (C.c_double * len(scale_factors))(*[float(f) for f in scale_factors])
         ws = torch.empty(nbytes // 4, dtype=torch.float32, device=self.device)
         z = torch.empty((n, VIT_DIM), device=self.device, dtype=torch.float32)
@@ -544,7 +537,7 @@ class Context:
 
     def vit_backward(self, params: Sequence[torch.Tensor], ws: torch.Tensor, grad_z: torch.Tensor) -> List[torch.Tensor]:
         """d(sum(grad_z * z)) / d params for the forward held in `ws`."""
-        arr = self._vit_array(params, "parameter")
+        arr = self._tensor_array(params, PDB_VIT_NUM_TENSORS, "parameter")
         _check_dev(grad_z, "grad_z", self.device)
         grads = [torch.empty_like(p) for p in params]
         garr = (C.c_void_p * len(grads))(*[C.c_void_p(g.data_ptr()) for g in grads])

@@ -55,7 +55,9 @@ struct Context {
   VitWeights* vit = nullptr;
   void* vit_ws = nullptr;
   size_t vit_ws_bytes = 0;
-  size_t attr_vit_att[4] = {0, 0, 0, 0};
+  size_t attr_vit_att[2] = {0, 0};  // the forward attention kernel's copy in api_vit.cu / api_vit_train.cu
+  size_t attr_vit_att_bwd = 0;      // backbone attention backward (csrc/api_vit_train.cu)
+  bool attr_train_att = false;      // denoiser training attention, forward and backward (csrc/api_train.cu)
   int ggs_layout = 1;       // stream layout of match sets packed on this context (ggs_layout.cuh): 0 plain, 1 paired (default)
   int denoiser_engine = 0;  // 0 auto, 1 fp32 persistent kernel, 2 wgmma/TMA tiles (TF32)
   // optional per-kernel timing (bench.py roofline): event pairs per launch, kind 0 = GGS, 1 = denoiser

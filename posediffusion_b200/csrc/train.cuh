@@ -1,20 +1,18 @@
 // Training kernels of the denoiser (csrc/api_train.cu): p_losses forward with saved activations, and its backward.
 // Projections run on the tensor-core linear layer (tc_linear.cuh); everything here is fp32 element-wise, LayerNorm,
-// attention and reduction code.  Every reduction over tokens is split into a fixed number of token chunks and the chunk
-// partials are added in chunk order: no floating-point atomics, the same inputs give bit-identical gradients.
-// The backbone's training path (csrc/api_vit_train.cu) uses the LayerNorm, transpose and column-sum kernels too; the kernels sit
-// in an anonymous namespace so that each including translation unit owns its copy.
+// attention and reduction code that only the denoiser uses: dropout, the schedule, the time MLP, the feed row, attention, the
+// tail and the _first / time-MLP gradients.  What the backbone's training path needs too (LayerNorm, transposes, column sums,
+// the linear-layer backward) is in csrc/train_common.cuh, with the rules that make gradients bit-identical from run to run.
 #pragma once
 #include <cstdint>
 
-#include "common.cuh"
 #include "posediff_b200.h"
+#include "train_common.cuh"
 
 namespace pdb {
 
 constexpr int kTrainMaxFrames = 64;  // attention backward keeps Q, K, V, dO and two N x N tiles of one (sequence, head) in smem
 constexpr int kFeedPad = 704;        // 702 feed columns (harmonic | t-embedding | z | pivot) zero-padded to a multiple of 64
-constexpr int kRedChunks = 128;      // token chunks of the deterministic column reductions
 
 // ---- dropout: Philox4x32-10 keyed by the 64-bit seed, counter = (element >> 2, element >> 34, layer << 8 | site, 0) ------------
 // The same function builds the masks in the forward kernels, the backward kernels (masks are recomputed, never stored) and
@@ -124,36 +122,6 @@ __global__ void train_feed_kernel(const __grid_constant__ TrainSched sc, const f
   }
 }
 
-// LayerNorm over C columns (biased variance), one warp per row; stats[row] = {mean, rstd}
-template <int C>
-__global__ void train_ln_fwd_kernel(const float* __restrict__ x, const float* __restrict__ g, const float* __restrict__ bta, int S,
-                                    float eps, float* __restrict__ y, float* __restrict__ stats) {
-  constexpr int P = C / 32;
-  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (row >= S) return;
-  const float* xr = x + (size_t)row * C;
-  float v[P], sum = 0.f;
-#pragma unroll
-  for (int i = 0; i < P; ++i) {
-    v[i] = xr[lane + 32 * i];
-    sum += v[i];
-  }
-  const float mean = warp_sum(sum) * (1.0f / C);
-  float sq = 0.f;
-#pragma unroll
-  for (int i = 0; i < P; ++i) sq += (v[i] - mean) * (v[i] - mean);
-  const float rstd = 1.0f / sqrtf(warp_sum(sq) * (1.0f / C) + eps);
-#pragma unroll
-  for (int i = 0; i < P; ++i) {
-    const int c = lane + 32 * i;
-    y[(size_t)row * C + c] = (v[i] - mean) * rstd * g[c] + bta[c];
-  }
-  if (lane == 0) {
-    stats[2 * row] = mean;
-    stats[2 * row + 1] = rstd;
-  }
-}
-
 // out = (res ? res : 0) + a * keep * scale * (gate ? gate > 0 : 1) over an [S, cols] array; mask element = flat index
 __global__ void train_dropout_kernel(const float* a, const float* res, const float* gate, float* out, long long n, DropCfg d, int layer,
                                      int site) {
@@ -238,17 +206,10 @@ __global__ void train_tail_fwd_kernel(const __grid_constant__ TrainSched sc, con
                                       float* __restrict__ loss, float* __restrict__ x0) {
   const int s = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (s >= S) return;
-  float v[4], sum = 0.f;
+  float v[4], mean, rstd;
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    v[i] = u[(size_t)s * 128 + lane + 32 * i];
-    sum += v[i];
-  }
-  const float mean = warp_sum(sum) * (1.0f / 128);
-  float sq = 0.f;
-#pragma unroll
-  for (int i = 0; i < 4; ++i) sq += (v[i] - mean) * (v[i] - mean);
-  const float rstd = 1.0f / sqrtf(warp_sum(sq) * (1.0f / 128) + 1e-5f);
+  for (int i = 0; i < 4; ++i) v[i] = u[(size_t)s * 128 + lane + 32 * i];
+  ln_row_stats(v, 1e-5f, mean, rstd);
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int c = lane + 32 * i;
@@ -276,47 +237,6 @@ __global__ void train_tail_fwd_kernel(const __grid_constant__ TrainSched sc, con
 }
 
 // ---- backward ----------------------------------------------------------------------------------------------------------------
-// out[C, Rp] = in[R, C]^T, rows R..Rp-1 of the result zero (token padding of the weight-gradient GEMMs)
-__global__ void train_transpose_kernel(const float* __restrict__ in, int R, int C, int Rp, float* __restrict__ out) {
-  __shared__ float tile[32][33];
-  const int r0 = blockIdx.y * 32, c0 = blockIdx.x * 32;
-  for (int k = threadIdx.y; k < 32; k += blockDim.y) {
-    const int r = r0 + k, c = c0 + threadIdx.x;
-    tile[k][threadIdx.x] = (r < R && c < C) ? in[(size_t)r * C + c] : 0.f;
-  }
-  __syncthreads();
-  for (int k = threadIdx.y; k < 32; k += blockDim.y) {
-    const int c = c0 + k, r = r0 + threadIdx.x;
-    if (c < C && r < Rp) out[(size_t)c * Rp + r] = tile[threadIdx.x][k];
-  }
-}
-
-// copy rows x cols of src (leading dimension lds) into dst (leading dimension ldd), columns cols..ldd-1 of dst zero
-__global__ void train_copy_cols_kernel(const float* __restrict__ src, int lds, int rows, int cols, float* __restrict__ dst, int ldd) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (long long)rows * ldd) return;
-  const int r = (int)(i / ldd), c = (int)(i % ldd);
-  dst[i] = c < cols ? src[(size_t)r * lds + c] : 0.f;
-}
-
-// deterministic column sums, stage 1: partial[chunk][c] = sum over the chunk's rows of A[row][c] (rows in order)
-__global__ void train_colsum_partial_kernel(const float* __restrict__ A, int S, int C, float* __restrict__ partial) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x, chunk = blockIdx.y;
-  if (c >= C) return;
-  const int per = (S + kRedChunks - 1) / kRedChunks, s0 = chunk * per, s1 = min(S, s0 + per);
-  float acc = 0.f;
-  for (int s = s0; s < s1; ++s) acc += A[(size_t)s * C + c];
-  partial[(size_t)chunk * C + c] = acc;
-}
-// stage 2: out[c] = sum over chunks in chunk order
-__global__ void train_chunk_sum_kernel(const float* __restrict__ partial, int chunks, int C, float* __restrict__ out) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  float acc = 0.f;
-  for (int k = 0; k < chunks; ++k) acc += partial[(size_t)k * C + c];
-  out[c] = acc;
-}
-
 // tail backward, one warp per token: deps = grad_loss * dloss/deps - sqrt_recipm1(t) * grad_x0 (stored [S,9] for the _last.3
 // gradients); dr = deps W3; d(LN out) = dr * (r > 0)
 __global__ void train_tail_bwd_kernel(const __grid_constant__ TrainSched sc, const float* __restrict__ diff, const float* __restrict__ gl,
@@ -359,36 +279,6 @@ __global__ void train_w3_partial_kernel(const float* __restrict__ deps, const fl
   }
 #pragma unroll
   for (int o = 0; o < 9; ++o) partial[(size_t)chunk * 1152 + o * 128 + k] = acc[o];
-}
-
-// LayerNorm backward, warp per row: dx = rstd (g - mean(g) - xhat mean(g xhat)), g = dy * gamma; out = (res ? res : 0) + dx;
-// prod = dy * xhat (its column sums are the gamma gradient)
-template <int C>
-__global__ void train_ln_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ stats,
-                                    const float* __restrict__ gamma, const float* res, int S, float* out, float* __restrict__ prod) {
-  constexpr int P = C / 32;
-  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (row >= S) return;
-  const float mean = stats[2 * row], rstd = stats[2 * row + 1];
-  float xh[P], g[P], sg = 0.f, sgx = 0.f;
-#pragma unroll
-  for (int i = 0; i < P; ++i) {
-    const int c = lane + 32 * i;
-    const float d = dy[(size_t)row * C + c];
-    xh[i] = (x[(size_t)row * C + c] - mean) * rstd;
-    g[i] = d * gamma[c];
-    prod[(size_t)row * C + c] = d * xh[i];
-    sg += g[i];
-    sgx += g[i] * xh[i];
-  }
-  sg = warp_sum(sg) * (1.0f / C);
-  sgx = warp_sum(sgx) * (1.0f / C);
-#pragma unroll
-  for (int i = 0; i < P; ++i) {
-    const int c = lane + 32 * i;
-    const float dx = rstd * (g[i] - sg - xh[i] * sgx);
-    out[(size_t)row * C + c] = res ? res[(size_t)row * C + c] + dx : dx;
-  }
 }
 
 // attention backward of one (sequence, head); writes the q / k / v column blocks of dqkv [S, 1536]

@@ -1,9 +1,10 @@
 // Training kernels of the DINO ViT-S/16 backbone (csrc/api_vit_train.cu): what the backward needs beyond the shared pieces of
-// csrc/vit.cuh (patchify, attention forward, head) and csrc/train.cuh (LayerNorm forward / backward, transposes, column sums).
+// csrc/vit.cuh (patchify, attention forward, head) and csrc/train_common.cuh (LayerNorm forward / backward, the linear-layer
+// backward, column sums).
 // All fp32 CUDA-core code; the projections and their gradients run on the tensor-core linear layer.  Every reduction over tokens
 // or images is a fixed-order sum: no floating-point atomics, two runs give bit-identical gradients.
 #pragma once
-#include "train.cuh"
+#include "train_common.cuh"
 #include "vit.cuh"
 
 namespace {
@@ -54,18 +55,10 @@ __global__ void vit_head_bwd_kernel(const float* __restrict__ X, VitHeadArgs a, 
   const int s = item / n_images, n = item - s * n_images;
   const size_t row = (size_t)(a.row0[s] + n * a.tokens[s]);
   constexpr int P = kVitDim / 32;
-  float v[P], sum = 0.f;
+  float v[P], g[P], m, rstd, mg, mgx;
 #pragma unroll
-  for (int i = 0; i < P; ++i) {
-    v[i] = X[row * kVitDim + lane + 32 * i];
-    sum += v[i];
-  }
-  const float m = warp_sum(sum) * (1.0f / kVitDim);
-  float sq = 0.f;
-#pragma unroll
-  for (int i = 0; i < P; ++i) sq += (v[i] - m) * (v[i] - m);
-  const float rstd = 1.0f / sqrtf(warp_sum(sq) * (1.0f / kVitDim) + kVitLnEps);
-  float g[P], sg = 0.f, sgx = 0.f;
+  for (int i = 0; i < P; ++i) v[i] = X[row * kVitDim + lane + 32 * i];
+  ln_row_stats(v, kVitLnEps, m, rstd);
 #pragma unroll
   for (int i = 0; i < P; ++i) {
     const int c = lane + 32 * i;
@@ -74,13 +67,10 @@ __global__ void vit_head_bwd_kernel(const float* __restrict__ X, VitHeadArgs a, 
     g[i] = dy * gamma[c];
     prod[(size_t)item * kVitDim + c] = dy * v[i];
     dy_rows[(size_t)item * kVitDim + c] = dy;
-    sg += g[i];
-    sgx += g[i] * v[i];
   }
-  sg = warp_sum(sg) * (1.0f / kVitDim);
-  sgx = warp_sum(sgx) * (1.0f / kVitDim);
+  ln_row_bwd_means(v, g, mg, mgx);
 #pragma unroll
-  for (int i = 0; i < P; ++i) dX[row * kVitDim + lane + 32 * i] = rstd * (g[i] - sg - v[i] * sgx);
+  for (int i = 0; i < P; ++i) dX[row * kVitDim + lane + 32 * i] = ln_row_dx(v[i], g[i], mg, mgx, rstd);
 }
 
 // ---- attention backward of one (sequence, head), L <= 256 tokens, head width 64, fp32 in shared memory ----

@@ -300,6 +300,23 @@ def test_out_of_range_timesteps_are_refused():
         ctx.train_backward(params, ws, torch.ones_like(x), None)
 
 
+def test_launch_count_is_the_number_of_kernels_enqueued():
+    """Forward: 5 feed kernels, 10 per layer, 2 for the tail.  Backward: 17 for the tail, 42 per layer (each linear layer's input,
+    weight and bias gradients are 2 + 3 + 2), 10 for _first and the time MLP; dL/dz adds a padded copy, a transpose and a GEMM."""
+    dif, _ = make_diffuser()
+    ctx = _native.Context.get(DEV)
+    params = dif.model.ordered_parameters()
+    x, t, noise, z = [v.to(DEV) for v in inputs(3, 7)]
+    counts = [ctx.launch_count]
+    ws, *_ = ctx.train_forward(params, x, t.int(), noise, z, 0.1, 5, "l1")
+    counts.append(ctx.launch_count)
+    ctx.train_backward(params, ws, torch.ones_like(x), None)
+    counts.append(ctx.launch_count)
+    ctx.train_backward(params, ws, torch.ones_like(x), None, grad_z=torch.empty_like(z))
+    counts.append(ctx.launch_count)
+    assert [b - a for a, b in zip(counts, counts[1:])] == [5 + 8 * 10 + 2, 17 + 8 * 42 + 10, 17 + 8 * 42 + 10 + 3]
+
+
 # ---- the reference's own training step and camera encoding (tests/golden/train.npz, oracle/make_golden_train.py) -------------
 from oracle.make_golden_train import CASES as GOLDEN_CASES, sample_index  # noqa: E402
 

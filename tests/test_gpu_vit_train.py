@@ -100,6 +100,24 @@ def test_two_runs_are_bit_identical_and_second_backward_raises():
         z.sum().backward()
 
 
+@pytest.mark.parametrize("h,w,scales,resampled", [(224, 224, DEFAULT, 2), (224, 232, DEFAULT, 3), (224, 224, (1, 1 / 2, 1 / 3, 1.1), 3)])
+def test_launch_count_is_the_number_of_kernels_enqueued(h, w, scales, resampled):
+    """Forward: one position-table kernel per resampled scale, patchify and position add per scale, the patch GEMM, 8 per block,
+    the head.  Backward: 5 for the head, per block 42 plus one attention backward per scale (each linear layer's input, weight and
+    bias gradients are 2 + 3 + 2), then the patch weight (3), one position sum per scale and the position gradient."""
+    ext, _ = make_extractor(scales=scales)
+    ctx = _native.Context.get(DEV)
+    params = list(ext._net.parameters())
+    k = len(scales)
+    before = ctx.launch_count
+    ws, z = ctx.vit_train_forward(params, images(2, h, w).to(DEV), scales)
+    mid = ctx.launch_count
+    ctx.vit_backward(params, ws, torch.ones_like(z))
+    after = ctx.launch_count
+    assert mid - before == resampled + 2 * k + 1 + 12 * 8 + 1
+    assert after - mid == 5 + 12 * (42 + k) + 3 + k + 1
+
+
 def test_frozen_or_no_grad_calls_take_the_inference_path():
     ext, _ = make_extractor()
     img = images(2).to(DEV)
