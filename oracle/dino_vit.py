@@ -6,7 +6,8 @@ restates the published algorithm of that repository's `vision_transformer.py` (`
 
   * patch embedding: Conv2d(3, 384, kernel 16, stride 16) -> tokens in (row, column) order, class token prepended;
   * position embedding [1, 197, 384], bicubically resampled for other resolutions with the `+0.1` scale-factor trick
-    (`interpolate_pos_encoding`), i.e. `F.interpolate(..., scale_factor=((h//16 + 0.1)/14, (w//16 + 0.1)/14), mode="bicubic")`;
+    (`interpolate_pos_encoding`), i.e. `F.interpolate(..., scale_factor=((h//16 + 0.1)/14, (w//16 + 0.1)/14), mode="bicubic")`,
+    applied here as the matrix that call is on the 196 grid cells (`resample_matrix`), so that autograd gives its transpose;
   * 12 pre-norm blocks: x += proj(MHSA(LN(x))), x += fc2(GELU(fc1(LN(x)))), 6 heads of 64, qkv with bias, LN eps 1e-6;
   * final LayerNorm, the class token is the feature (head = Identity).
 
@@ -18,6 +19,7 @@ multi-scale wrapper around it is the reference's own `MultiScaleImageFeatureExtr
 """
 from __future__ import annotations
 
+import functools
 import math
 
 import torch
@@ -25,6 +27,22 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 EMBED, DEPTH, HEADS, PATCH, MLP = 384, 12, 6, 16, 1536
+
+
+GRID0 = 14  # the stored position grid
+
+
+@functools.lru_cache(maxsize=None)
+def resample_matrix(gh: int, gw: int) -> torch.Tensor:
+    """R_s [gh*gw, 196], float64: interpolate_pos_encoding's bicubic resampling of the 14x14 grid at scale (grid + 0.1) / 14,
+    row-major cells, read off F.interpolate on the CPU applied to the 196 basis grids.  The table is then a product, whose
+    autograd is R_s^T.  Autograd through F.interpolate itself is not: when the grid keeps its 14x14 size (a non-square image)
+    torch's bicubic backward copies the gradient through as if the resampling were the identity (9.5 % off R_s^T), and the CUDA
+    forward copies the grid."""
+    basis = torch.eye(GRID0 * GRID0, dtype=torch.float64).reshape(-1, 1, GRID0, GRID0)
+    out = F.interpolate(basis, scale_factor=((gh + 0.1) / GRID0, (gw + 0.1) / GRID0), mode="bicubic")
+    assert tuple(out.shape[-2:]) == (gh, gw)
+    return out.reshape(GRID0 * GRID0, gh * gw).T.contiguous()
 
 
 class _Attention(nn.Module):
@@ -93,12 +111,9 @@ class DinoViTSmall16(nn.Module):
         n0 = self.pos_embed.shape[1] - 1
         if n_patches == n0 and w == h:
             return self.pos_embed
-        side = int(math.sqrt(n0))
-        h0, w0 = h // PATCH + 0.1, w // PATCH + 0.1
-        grid = self.pos_embed[:, 1:].reshape(1, side, side, EMBED).permute(0, 3, 1, 2)
-        grid = F.interpolate(grid, scale_factor=(h0 / side, w0 / side), mode="bicubic")
-        assert int(h0) == grid.shape[-2] and int(w0) == grid.shape[-1]
-        return torch.cat((self.pos_embed[:, :1], grid.permute(0, 2, 3, 1).reshape(1, -1, EMBED)), dim=1)
+        assert n0 == GRID0 * GRID0, n0
+        R = resample_matrix(h // PATCH, w // PATCH).to(self.pos_embed.device, self.pos_embed.dtype)
+        return torch.cat((self.pos_embed[:, :1], (R @ self.pos_embed[0, 1:])[None]), dim=1)
 
     def prepare_tokens(self, img):
         B, _, h, w = img.shape

@@ -56,27 +56,31 @@ def _linear(x, w, b, mode):
 def _drop(x, masks, key, p):
     if masks is None:
         return x
-    return x * masks[key].to(x.dtype) / (1.0 - p)
+    return x * masks[key].to(x.device, x.dtype) / (1.0 - p)
 
 
 def forward(params: Dict[str, torch.Tensor], x_start, t, noise, z, loss_type: str = "l1", masks: Optional[Dict[Tuple[int, int], torch.Tensor]] = None,
-            p: float = 0.0, tf32: Optional[str] = None, dtype: torch.dtype = torch.float64) -> Dict[str, torch.Tensor]:
+            p: float = 0.0, tf32: Optional[str] = None, dtype: torch.dtype = torch.float64, device="cpu") -> Dict[str, torch.Tensor]:
     """params: the 108 denoiser tensors by state_dict name (float64, may require grad); x_start / noise [B,N,9], t [B] int, z [B,N,384].
-    masks[(layer, site)]: keep masks, site 0 [B,4,N,N], sites 1 and 3 [B,N,512], site 2 [B,N,1024]."""
+    masks[(layer, site)]: keep masks, site 0 [B,4,N,N], sites 1 and 3 [B,N,512], site 2 [B,N,1024].  Runs on `device` (params
+    must be there); the float32 harmonic and timestep features are computed on the CPU whatever the device, so that every device
+    evaluates the same features."""
     P = params
     dt = dtype
-    sched = {k: v.to(dt) for k, v in diffusion_schedule().items()}
+    sched = {k: v.to(device, dt) for k, v in diffusion_schedule().items()}
     B, N, _ = x_start.shape
     tl = t.long().cpu()
-    col = lambda name: sched[name][tl].view(B, 1, 1)  # noqa: E731
-    x_start, noise, z = x_start.to(dt), noise.to(dt), z.to(dt)
+    td = tl.to(device)
+    col = lambda name: sched[name][td].view(B, 1, 1)  # noqa: E731
+    x_start, noise, z = x_start.to(device, dt), noise.to(device, dt), z.to(device, dt)
     x_t = col("sqrt_alphas_cumprod") * x_start + col("sqrt_one_minus_alphas_cumprod") * noise
-    tf = timestep_features(tl).to(dt)
+    tf = timestep_features(tl).to(device, dt)
     u1 = tf @ P["time_embed.linear.0.weight"].T + P["time_embed.linear.0.bias"]
     temb = F.silu(u1) @ P["time_embed.linear.2.weight"].T + P["time_embed.linear.2.bias"]
-    pivot = torch.zeros(B, N, 1, dtype=dt)
+    pivot = torch.zeros(B, N, 1, dtype=dt, device=device)
     pivot[:, 0] = 1.0
-    feed = torch.cat([harmonic_features(x_t.float()).to(dt), temb[:, None, :].expand(B, N, -1), z, pivot], dim=-1)
+    harm = harmonic_features(x_t.float().cpu()).to(device, dt)
+    feed = torch.cat([harm, temb[:, None, :].expand(B, N, -1), z, pivot], dim=-1)
     h = _linear(feed, P["_first.weight"], P["_first.bias"], tf32)
     scale = 1.0 / math.sqrt(D_MODEL // HEADS)
     for l in range(LAYERS):
@@ -106,17 +110,61 @@ def forward(params: Dict[str, torch.Tensor], x_start, t, noise, z, loss_type: st
 
 def loss_and_grads(state: Dict[str, torch.Tensor], x_start, t, noise, z, grad_loss, grad_x0=None, loss_type: str = "l1", masks=None,
                    p: float = 0.0, tf32: Optional[str] = None, names: Optional[Sequence[str]] = None,
-                   dtype: torch.dtype = torch.float64):
-    """forward() plus d(sum(grad_loss * loss) + sum(grad_x0 * x_0_pred)) / d params on the CPU, in float64 unless `dtype` says
-    otherwise (float32 gives the distance an fp32 evaluation of the same step has from float64)."""
-    params = {k: v.detach().to("cpu", dtype).requires_grad_(True) for k, v in state.items()}
-    out = forward(params, x_start.cpu(), t.cpu(), noise.cpu(), z.cpu(), loss_type, masks, p, tf32, dtype)
-    total = (out["loss"] * grad_loss.cpu().to(dtype)).sum()
+                   dtype: torch.dtype = torch.float64, device="cpu"):
+    """forward() plus d(sum(grad_loss * loss) + sum(grad_x0 * x_0_pred)) / d params on `device` (default the CPU), in float64
+    unless `dtype` says otherwise (float32 gives the distance an fp32 evaluation of the same step has from float64)."""
+    params = {k: v.detach().to(device, dtype).requires_grad_(True) for k, v in state.items()}
+    out = forward(params, x_start, t, noise, z, loss_type, masks, p, tf32, dtype, device)
+    total = (out["loss"] * grad_loss.to(device, dtype)).sum()
     if grad_x0 is not None:
-        total = total + (out["x_0_pred"] * grad_x0.cpu().to(dtype)).sum()
+        total = total + (out["x_0_pred"] * grad_x0.to(device, dtype)).sum()
     names = list(names or params)
     grads = torch.autograd.grad(total, [params[n] for n in names], allow_unused=True)
     return {k: v.detach() for k, v in out.items()}, {n: (g if g is not None else torch.zeros_like(params[n])) for n, g in zip(names, grads)}
+
+
+def dropout_masks(seed: int, b0: int, b1: int, frames: int, p: float) -> Dict[Tuple[int, int], torch.Tensor]:
+    """The training kernels' keep masks (forward()'s `masks`) of sequences b0 .. b1-1 of a batch of `frames`-frame sequences:
+    each site's mask is indexed by the flat element index of the whole batch, so this range starts at b0 * 4 * N^2 (attention
+    weights), b0 * N * 512 (sites 1 and 3) and b0 * N * 1024 (site 2).  Drawn by the library's host copy of the Philox function."""
+    from posediffusion_b200._native import dropout_mask_host
+
+    n, masks = b1 - b0, {}
+    for l in range(LAYERS):
+        for site, per_seq in ((0, (HEADS, frames, frames)), (1, (frames, D_MODEL)), (2, (frames, 2 * D_MODEL)), (3, (frames, D_MODEL))):
+            size = math.prod(per_seq)
+            keep = dropout_mask_host(seed, l, site, b0 * size, n * size, p)
+            masks[(l, site)] = torch.from_numpy(keep.reshape((n,) + per_seq).astype("float64"))
+    return masks
+
+
+def loss_and_grads_chunked(state: Dict[str, torch.Tensor], x_start, t, noise, z, grad_loss, grad_x0=None, loss_type: str = "l1",
+                           p: float = 0.0, seed: Optional[int] = None, tf32: Optional[str] = None, chunk: int = 64,
+                           dtype: torch.dtype = torch.float64, device="cpu", offset: int = 0):
+    """loss_and_grads() of a large batch, `chunk` sequences at a time, plus dL/dz: (outputs [B,N,9] on the CPU, parameter
+    gradients summed over chunks in `dtype` on the CPU, dz [B,N,384] on the CPU).  With p > 0 each chunk takes the masks the
+    kernels draw with `seed` at its own offsets (dropout_masks); `offset` is the index of x_start[0] in the batch the kernels
+    ran (the last sequences of a large step are checked by passing them alone)."""
+    params = {k: v.detach().to(device, dtype).requires_grad_(True) for k, v in state.items()}
+    names = list(params)
+    B = x_start.shape[0]
+    outs, dzs, grads = [], [], None
+    for b0 in range(0, B, chunk):
+        b1 = min(B, b0 + chunk)
+        sl = slice(b0, b1)
+        masks = dropout_masks(seed, offset + b0, offset + b1, x_start.shape[1], p) if p > 0 else None
+        zz = z[sl].detach().to(device, dtype).requires_grad_(True)
+        out = forward(params, x_start[sl], t[sl], noise[sl], zz, loss_type, masks, p, tf32, dtype, device)
+        total = (out["loss"] * grad_loss[sl].to(device, dtype)).sum()
+        if grad_x0 is not None:
+            total = total + (out["x_0_pred"] * grad_x0[sl].to(device, dtype)).sum()
+        g = torch.autograd.grad(total, [params[n] for n in names] + [zz], allow_unused=True)
+        gp = [gi if gi is not None else torch.zeros_like(params[n]) for n, gi in zip(names, g[:-1])]
+        grads = gp if grads is None else [a + b for a, b in zip(grads, gp)]
+        outs.append({k: v.detach().cpu() for k, v in out.items()})
+        dzs.append(g[-1].cpu())
+    out = {k: torch.cat([o[k] for o in outs]) for k in outs[0]}
+    return out, {n: gi.cpu() for n, gi in zip(names, grads)}, torch.cat(dzs)
 
 
 def matrix_to_quaternion(matrix: torch.Tensor) -> torch.Tensor:

@@ -20,7 +20,7 @@ from typing import Dict, List, Optional, Sequence
 import torch
 import torch.nn.functional as F
 
-from oracle.dino_vit import EMBED, HEADS, PATCH, RESNET_MEAN, RESNET_STD
+from oracle.dino_vit import EMBED, HEADS, PATCH, RESNET_MEAN, RESNET_STD, resample_matrix
 from oracle.train_oracle import tf32_round
 
 GRID0 = 14
@@ -36,12 +36,13 @@ def _rna(x):
 
 
 class VitF64:
-    """Evaluator over one DinoViTSmall16 state_dict (hub parameter names)."""
+    """Evaluator over one DinoViTSmall16 state_dict (hub parameter names), on `device` (default the CPU)."""
 
-    def __init__(self, state: Dict[str, torch.Tensor], dtype: torch.dtype = torch.float64):
+    def __init__(self, state: Dict[str, torch.Tensor], dtype: torch.dtype = torch.float64, device="cpu"):
         self.dtype = dtype
-        self.p = {k: v.detach().to("cpu", dtype) for k, v in state.items()}
-        p32 = {k: v.detach().to("cpu", torch.float32) for k, v in state.items()}
+        self.device = torch.device(device)
+        self.p = {k: v.detach().to(device, dtype) for k, v in state.items()}
+        p32 = {k: v.detach().to(device, torch.float32) for k, v in state.items()}
         self.folded = {}  # (block, "qkv" | "fc1") -> (W', colsum, b') as the device holds them, widened
         for l in range(12):
             pre = f"blocks.{l}."
@@ -93,15 +94,13 @@ class VitF64:
         pos = self.p["pos_embed"][0]
         if gh * gw == GRID0 * GRID0 and h == w:
             return pos
-        grid = pos[1:].reshape(1, GRID0, GRID0, EMBED).permute(0, 3, 1, 2)
-        grid = F.interpolate(grid, scale_factor=((gh + 0.1) / GRID0, (gw + 0.1) / GRID0), mode="bicubic")
-        assert tuple(grid.shape[-2:]) == (gh, gw)
-        return torch.cat([pos[:1], grid[0].permute(1, 2, 0).reshape(-1, EMBED)])
+        R = resample_matrix(gh, gw).to(pos.device, pos.dtype)
+        return torch.cat([pos[:1], R @ pos[1:]])
 
     def pyramid(self, image_rgb: torch.Tensor, scale_factors: Sequence[float]) -> List[torch.Tensor]:
-        mean = torch.tensor(RESNET_MEAN, dtype=self.dtype).view(1, 3, 1, 1)
-        std = torch.tensor(RESNET_STD, dtype=self.dtype).view(1, 3, 1, 1)
-        normed = (image_rgb.to("cpu", self.dtype) - mean) / std
+        mean = torch.tensor(RESNET_MEAN, dtype=self.dtype, device=self.device).view(1, 3, 1, 1)
+        std = torch.tensor(RESNET_STD, dtype=self.dtype, device=self.device).view(1, 3, 1, 1)
+        normed = (image_rgb.to(self.device, self.dtype) - mean) / std
         return [normed if f == 1 else F.interpolate(normed, scale_factor=f, mode="bilinear", align_corners=False) for f in scale_factors]
 
     def prepare_tokens(self, img: torch.Tensor, mode=None) -> torch.Tensor:

@@ -21,8 +21,9 @@ from oracle.vit_f64 import VitF64
 class _VitGrad(VitF64):
     """VitF64 over parameters that require grad; `mode` is None (exact) or "tf32"."""
 
-    def __init__(self, params: Dict[str, torch.Tensor], dtype):
+    def __init__(self, params: Dict[str, torch.Tensor], dtype, device="cpu"):
         self.dtype = dtype
+        self.device = torch.device(device)
         self.p = params
         self.folded = {}
 
@@ -44,9 +45,23 @@ class _VitGrad(VitF64):
 
 
 def features_and_grads(state: Dict[str, torch.Tensor], image_rgb: torch.Tensor, scale_factors: Sequence[float], grad_z: torch.Tensor,
-                       tf32: bool = False, dtype: torch.dtype = torch.float64):
-    """(z [n,384], {name: d(sum(grad_z * z)) / d tensor}) on the CPU, in float64 unless `dtype` says otherwise."""
-    params = {k: v.detach().to("cpu", dtype).requires_grad_(True) for k, v in state.items()}
-    z = _VitGrad(params, dtype).features(image_rgb, scale_factors, "tf32" if tf32 else None)
-    grads = torch.autograd.grad((z * grad_z.to("cpu", dtype)).sum(), list(params.values()))
+                       tf32: bool = False, dtype: torch.dtype = torch.float64, device="cpu"):
+    """(z [n,384], {name: d(sum(grad_z * z)) / d tensor}) on `device` (default the CPU), in float64 unless `dtype` says otherwise."""
+    params = {k: v.detach().to(device, dtype).requires_grad_(True) for k, v in state.items()}
+    z = _VitGrad(params, dtype, device).features(image_rgb, scale_factors, "tf32" if tf32 else None)
+    grads = torch.autograd.grad((z * grad_z.to(device, dtype)).sum(), list(params.values()))
     return z.detach(), dict(zip(params, grads))
+
+
+def features_and_grads_chunked(state: Dict[str, torch.Tensor], image_rgb: torch.Tensor, scale_factors: Sequence[float],
+                               grad_z: torch.Tensor, tf32: bool = False, chunk: int = 32, dtype: torch.dtype = torch.float64,
+                               device="cpu"):
+    """features_and_grads() of a large batch, `chunk` images at a time: (z [n,384], gradients summed over chunks in `dtype`),
+    both on the CPU.  Every image is its own sequence, so the chunks' z are the batch's and the gradients add up."""
+    zs, total = [], None
+    for i in range(0, image_rgb.shape[0], chunk):
+        z, g = features_and_grads(state, image_rgb[i:i + chunk], scale_factors, grad_z[i:i + chunk], tf32, dtype, device)
+        zs.append(z.cpu())
+        g = {k: v.cpu() for k, v in g.items()}
+        total = g if total is None else {k: total[k] + g[k] for k in g}
+    return torch.cat(zs), total

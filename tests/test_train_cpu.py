@@ -227,3 +227,48 @@ def test_camera_goldens_oracle_and_shim_round_trip(golden):
     torch.testing.assert_close(to.camera_to_pose_encoding(R, T, focal), want, rtol=0, atol=1e-6)
     assert (want[:, 3] >= 0).all()
     torch.testing.assert_close(quaternion_to_matrix(want[:, 3:7]), R, rtol=0, atol=2e-6)
+
+
+def _max_rel(a, b):
+    return float((a.double() - b.double()).norm() / b.double().norm().clamp(min=1e-30))
+
+
+def test_dropout_masks_of_consecutive_sequence_ranges_concatenate_to_one_call():
+    """A site's mask is indexed by the flat element index of the whole batch: host draws over consecutive offsets, and the
+    per-range masks of the oracle (sequences 0-1, 2-4 of 5), concatenate to the draw of the whole batch."""
+    seed, B, N, p = 0x1234_5678_9ABC, 5, 7, 0.1
+    whole = _native.dropout_mask_host(seed, 3, 2, 0, 1000, p)
+    parts = [_native.dropout_mask_host(seed, 3, 2, a, b - a, p) for a, b in ((0, 1), (1, 333), (333, 334), (334, 1000))]
+    assert np.array_equal(np.concatenate(parts), whole)
+    full = to.dropout_masks(seed, 0, B, N, p)
+    ranges = [to.dropout_masks(seed, 0, 2, N, p), to.dropout_masks(seed, 2, B, N, p)]
+    assert set(full) == {(l, s) for l in range(8) for s in range(4)}
+    for key, m in full.items():
+        assert torch.equal(torch.cat([r[key] for r in ranges]), m), key
+        assert 0 < m.mean().item() < 1, key
+    assert full[(0, 0)].shape == (B, 4, N, N) and full[(0, 2)].shape == (B, N, 1024) and full[(0, 3)].shape == (B, N, 512)
+
+
+@pytest.mark.parametrize("p", [0.0, 0.1])
+def test_chunked_oracle_equals_one_call(p):
+    """loss_and_grads_chunked (3 chunks of 2, 2 and 1 sequences, masks drawn per chunk) vs one loss_and_grads call over the
+    whole batch with the whole batch's masks; dL/dz against autograd of the same single call."""
+    state = syn.random_denoiser_state(6, 0.05)
+    B, N, seed = 5, 4, 99
+    g = torch.Generator().manual_seed(2)
+    x, noise = torch.randn(B, N, 9, generator=g), torch.randn(B, N, 9, generator=g)
+    t = torch.randint(0, 100, (B,), generator=g)
+    z = syn.random_features(B, N, 3)
+    gl, gx = torch.randn(B, N, 9, generator=g), torch.randn(B, N, 9, generator=g)
+    masks = to.dropout_masks(seed, 0, B, N, p) if p > 0 else None
+    out, grads, dz = to.loss_and_grads_chunked(state, x, t, noise, z, gl, gx, "l2", p=p, seed=seed, chunk=2)
+    ref, rgrads = to.loss_and_grads(state, x, t, noise, z, gl, gx, "l2", masks, p)
+    zz = z.double().requires_grad_(True)
+    o = to.forward({k: v.double() for k, v in state.items()}, x, t, noise, zz, "l2", masks, p)
+    rdz = torch.autograd.grad((o["loss"] * gl.double()).sum() + (o["x_0_pred"] * gx.double()).sum(), zz)[0]
+    for k in ("x_t", "x_0_pred", "loss", "eps"):
+        assert _max_rel(out[k], ref[k]) <= 1e-12, k
+    assert _max_rel(dz, rdz) <= 1e-12
+    assert set(grads) == set(rgrads)
+    for n in rgrads:
+        assert _max_rel(grads[n], rgrads[n]) <= 1e-12, n
