@@ -16,6 +16,8 @@
  *   pdb_sampson_eval       <- compute_sampson_distance + backward        (util/geometry_guided_sampling.py:129-172)
  *   pdb_ggs                <- geometry_guided_sampling (5 x GGS_optimize) (util/geometry_guided_sampling.py:14-126)
  *   pdb_sample_loop        <- GaussianDiffusion.sample / p_sample_loop   (models/gaussian_diffuser.py:285-306)
+ *   pdb_sample_loop_ddim   <- the fewer-step sampling the reference's `sampling_timesteps` names but never built (:79, :150-154,
+ *                             :303-306): a DDIM prefix in k < 100 steps, then the same guided DDPM + GGS tail
  *   pdb_sample_loop_host   <- the same call with HOST buffers (demo.py:108 as a user sees it: features and
  *                             matches on the host, poses back on the host)
  *   pdb_sample_loop_host_matches <- the same call starting from the reference's matches_dict arrays (demo.py:94-108:
@@ -125,6 +127,17 @@ int pdb_debug_tc_linear(pdb_context* ctx, const float* x_dev, const float* w_dev
  * alphas_cumprod}. */
 int pdb_schedule_table(float* out, double beta_1, double beta_T);
 
+/* DDIM step table (Song et al. 2021, eq. 12) for `steps` denoiser evaluations of which the last `guide_below` (g) are guided:
+ * the unguided prefix takes k = steps - g strided steps, 1 <= k <= 100 - g, tau_j = (g - 1) + floor(j * (100 - g) / k), entry i
+ * jumping tau_{k-i} -> tau_{k-i-1} (the last lands on x_{g-1}, or on x0 when g = 0).  HOST-ONLY, float64 arithmetic cast to float32:
+ * t_out[steps] = the timestep each entry evaluates the network at; coef_out[steps][8]: prefix entries {a_t, b_t, c1, c2, sigma, s,
+ * abar_t, abar_s} with x' = c1 * (a_t x - b_t eps) + c2 x + sigma * noise, sigma = eta sqrt((1-abar_s)/(1-abar_t)) sqrt(1 -
+ * abar_t/abar_s), c2 = sqrt(1 - abar_s - sigma^2) / sqrt(1 - abar_t), c1 = sqrt(abar_s) - c2 sqrt(abar_t), abar_{-1} = 1; entries
+ * k .. steps-1 are the pdb_schedule_table rows of timesteps g-1 .. 0 (the guided tail stays DDPM).  With k = 100 - g and eta = 1
+ * the prefix rows equal the DDPM posterior rows up to rounding.  PDB_ERR_INVALID for k out of range, eta < 0 or not finite, or
+ * an eta > 1 large enough to make 1 - abar_s - sigma^2 negative. */
+int pdb_ddim_table(int32_t steps, int32_t guide_below, double eta, double beta_1, double beta_T, int32_t* t_out, float* coef_out);
+
 /* ---- denoiser weights ---------------------------------------------------------------------------
  * `tensors[i]` (host or device, fp32, contiguous) in the order of the reference state_dict below
  * `diffuser.model.`:  time_embed.linear.0.{weight,bias}, time_embed.linear.2.{weight,bias},
@@ -202,6 +215,18 @@ int pdb_ggs(pdb_context* ctx, pdb_matches* const* problems, int32_t batch, float
 int pdb_sample_loop(pdb_context* ctx, const float* z_dev, const float* draws_dev, int32_t batch, int32_t frames,
                     pdb_matches* const* problems, int32_t n_problems, const pdb_ggs_config* cfg,
                     int32_t cond_start_step, float* pose_dev, float* trail_dev, pdb_ggs_stats* stats_dev, void* stream);
+
+/* pdb_sample_loop with a DDIM prefix: `steps` denoiser evaluations in all, of which g = clamp(cond_start_step, 0, 100) are the
+ * guided tail (exactly pdb_sample_loop's guided DDPM steps + GGS; problems / cfg / stats as there) and k = steps - g the unguided
+ * prefix on the pdb_ddim_table schedule.  draws_dev [1 + k, B, N, 9] when eta > 0 (draws[0] = x_T, draws[1 + i] = noise of
+ * prefix step i), [1, B, N, 9] when eta == 0 (x_T only).  trail_dev may be NULL, else [1 + steps, B, N, 9].  problems == NULL
+ * with cond_start_step > 0 runs the prefix alone and leaves x_{g-1} in pose_dev (a caller's own guidance takes over from there).
+ * PDB_ERR_INVALID before anything is enqueued for k out of range, a bad eta or a NULL draws pointer; PDB_ERR_LIMIT for frames >
+ * PDB_MAX_FRAMES.  The step table is copied (stream-ordered) into a buffer the context owns; concurrent loops on one context
+ * must share a stream. */
+int pdb_sample_loop_ddim(pdb_context* ctx, const float* z_dev, const float* draws_dev, int32_t batch, int32_t frames, int32_t steps,
+                         double eta, pdb_matches* const* problems, int32_t n_problems, const pdb_ggs_config* cfg,
+                         int32_t cond_start_step, float* pose_dev, float* trail_dev, pdb_ggs_stats* stats_dev, void* stream);
 
 /* The same with host buffers (pinned or pageable): copies z and the draws in, runs, copies pose (and the
  * optional trajectory / stats) out, synchronises the stream.  This is the end-to-end call bench.py times. */

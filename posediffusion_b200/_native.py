@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 import itertools
+import math
 import os
 import threading
 from typing import Dict, List, Optional, Sequence
@@ -71,6 +72,9 @@ EXPORTS = {
     "pdb_denoiser_engine": (C.c_int, [C.c_void_p, C.c_int32]),
     "pdb_debug_tc_linear": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "pdb_schedule_table": (C.c_int, [C.c_void_p, C.c_double, C.c_double]),
+    "pdb_ddim_table": (C.c_int, [C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_void_p, C.c_void_p]),
+    "pdb_sample_loop_ddim": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.POINTER(C.c_void_p),
+                                       C.c_int32, C.POINTER(GgsConfig), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "pdb_denoiser_load": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int32, C.c_void_p]),
     "pdb_denoiser_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "pdb_p_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -173,6 +177,30 @@ def schedule_table(beta_1: float = 1e-4, beta_T: float = 0.1) -> np.ndarray:
     if rc != 0:
         raise NativeError(f"pdb_schedule_table failed ({rc})")
     return out
+
+
+def ddim_table(steps: int, guide_below: int = 0, eta: float = 0.0, beta_1: float = 1e-4, beta_T: float = 0.1):
+    """(t [steps] int32, coef [steps, 8] float32): the DDIM step table of pdb_ddim_table -- `steps` denoiser evaluations, the last
+    `guide_below` of them guided DDPM steps (no GPU needed).  ValueError where the library refuses the arguments."""
+    n = max(int(steps), 1)
+    t = np.zeros(n, dtype=np.int32)
+    coef = np.zeros((n, 8), dtype=np.float32)
+    rc = load_library().pdb_ddim_table(int(steps), int(guide_below), float(eta), beta_1, beta_T, t.ctypes.data_as(C.c_void_p),
+                                       coef.ctypes.data_as(C.c_void_p))
+    if rc != 0:
+        raise ValueError(f"pdb_ddim_table refused steps={steps}, guide_below={guide_below}, eta={eta}")
+    return t, coef
+
+
+def ddim_check(steps: int, guided: int, eta: float) -> int:
+    """k = steps - guided unguided DDIM steps, or ValueError (the library's own check, mirrored so that nothing is enqueued)."""
+    k = int(steps) - int(guided)
+    if not 1 <= k <= NUM_TIMESTEPS - int(guided):
+        raise ValueError(f"sampling_timesteps={steps} with {guided} guided steps leaves {k} unguided DDIM steps; "
+                         f"1 .. {NUM_TIMESTEPS - int(guided)} are possible")
+    if not math.isfinite(float(eta)) or float(eta) < 0.0:
+        raise ValueError(f"eta={eta}: DDIM needs a finite eta >= 0")
+    return k
 
 
 def vit_pos_table(pos_embed: np.ndarray, grid_h: int, grid_w: int) -> np.ndarray:
@@ -671,6 +699,31 @@ class Context:
                                           trail.data_ptr() if want_trail else None,
                                           stats.data_ptr() if stats is not None else None, _stream_ptr(self.device)),
                  "pdb_sample_loop")
+        return pose, trail, stats
+
+    def sample_loop_ddim(self, z: torch.Tensor, draws: torch.Tensor, steps: int, eta: float, problems: Optional[Sequence[Matches]],
+                         cfg: Optional[Dict], cond_start_step: int, want_trail: bool = True, want_stats: bool = True):
+        """pdb_sample_loop_ddim: (pose, trail [1 + steps, B, N, 9] or None, stats).  draws [1 + k, B, N, 9] for eta > 0, [1, B, N, 9]
+        for eta == 0 (k = steps - guided).  Without problems and with cond_start_step > 0 only the prefix runs (pose = x_{g-1})."""
+        B, N, _ = z.shape
+        _check_dev(z, "z", self.device, (B, N, Z_DIM))
+        guided = max(0, min(int(cond_start_step), NUM_TIMESTEPS))
+        k = ddim_check(steps, guided, eta)
+        _check_dev(draws, "draws", self.device, (1 + k if eta > 0 else 1, B, N, TARGET_DIM))
+        if problems:
+            self._check_problems(problems, B, N)
+        pose = torch.empty(B, N, TARGET_DIM, device=self.device)
+        trail = torch.empty(1 + int(steps), B, N, TARGET_DIM, device=self.device) if want_trail else None
+        stats = None
+        if want_stats and problems and guided:
+            stats = torch.zeros(guided * B * GGS_STATS_DTYPE.itemsize, dtype=torch.uint8, device=self.device)
+        conf = ggs_config_struct(cfg) if problems else None
+        self._ok(self.lib.pdb_sample_loop_ddim(self.handle, z.data_ptr(), draws.data_ptr(), B, N, int(steps), float(eta),
+                                               self._problem_array(problems) if problems else None, len(problems) if problems else 0,
+                                               C.byref(conf) if conf is not None else None, int(cond_start_step), pose.data_ptr(),
+                                               trail.data_ptr() if want_trail else None,
+                                               stats.data_ptr() if stats is not None else None, _stream_ptr(self.device)),
+                 "pdb_sample_loop_ddim")
         return pose, trail, stats
 
     def sample_loop_host(self, z: np.ndarray, draws: np.ndarray, problems, cfg, cond_start_step: int,

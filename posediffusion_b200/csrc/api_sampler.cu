@@ -17,7 +17,7 @@ int enqueue_ggs(Context* ctx, pdb_matches* const* problems, int batch, int frame
                 pdb_ggs_stats* stats_dev, cudaStream_t st);
 int check_ggs_problems(Context* ctx, pdb_matches* const* problems, int batch, int frames);
 
-int enqueue_denoiser_tc(Context* ctx, DenoiserRun run, cudaStream_t st);
+int enqueue_denoiser_tc(Context* ctx, const DenoiserDev& dev, DenoiserRun run, cudaStream_t st);
 void vit_release(Context* ctx);
 }  // namespace pdb
 
@@ -104,7 +104,7 @@ int pick_token_tile(int tokens) {
 }
 
 template <int TS, bool kFlag>
-int launch_denoiser(Context* ctx, const DenoiserRun& run, int grid, cudaStream_t st) {
+int launch_denoiser(Context* ctx, const DenoiserDev& dev, const DenoiserRun& run, int grid, cudaStream_t st) {
   const size_t smem = denoiser_smem_bytes(TS, run.frames);
   if (smem > ctx->smem_optin) return ctx->fail(PDB_ERR_LIMIT, "denoiser needs %zu B shared memory", smem);
   size_t& attr_bytes = ctx->attr_den[(kFlag ? 8 : 0) + TS / 4 - 1];  // static shared memory counts against the opt-in limit: ask for what we use
@@ -124,15 +124,17 @@ int launch_denoiser(Context* ctx, const DenoiserRun& run, int grid, cudaStream_t
   cfg.numAttrs = 1;
   {
     ScopedTimer timer(ctx, st, 1);
-    PDB_CUDA(ctx, cudaLaunchKernelEx(&cfg, denoiser_kernel<TS, kFlag>, ctx->weights->dev, run));
+    PDB_CUDA(ctx, cudaLaunchKernelEx(&cfg, denoiser_kernel<TS, kFlag>, dev, run));
   }
   ctx->launches += 1;
   return PDB_OK;
 }
 
-// Fill the workspace pointers of `run` and launch steps t_hi..t_lo.
-int enqueue_denoiser(Context* ctx, DenoiserRun run, cudaStream_t st) {
+// Fill the workspace pointers of `run` and launch steps t_hi..t_lo.  `tables` (may be NULL: the loaded weights' own) is a copy of
+// the weight descriptor whose per-timestep rows -- `tproj` and `sched` -- are those of a DDIM step table (make_ddim_tables).
+int enqueue_denoiser(Context* ctx, DenoiserRun run, cudaStream_t st, const DenoiserDev* tables = nullptr) {
   if (!ctx->weights) return ctx->fail(PDB_ERR_STATE, "denoiser weights not loaded (pdb_denoiser_load)");
+  const DenoiserDev& dev = tables ? *tables : ctx->weights->dev;
   if (run.batch < 1 || run.frames < 1) return ctx->fail(PDB_ERR_INVALID, "empty batch");
   if (run.frames > PDB_MAX_FRAMES) return ctx->fail(PDB_ERR_LIMIT, "frames %d > PDB_MAX_FRAMES", run.frames);
   if (run.t_hi >= kT || run.t_lo < 0 || run.t_hi < run.t_lo) return ctx->fail(PDB_ERR_INVALID, "bad timestep range");
@@ -141,7 +143,7 @@ int enqueue_denoiser(Context* ctx, DenoiserRun run, cudaStream_t st) {
   // engine: exact-fp32 persistent kernel below kTcMinTokens tokens (latency bound), wgmma/TMA tiles (TF32 products) at or
   // above it (throughput bound).  ctx->denoiser_engine: 0 auto, 1 force fp32, 2 force tensor cores.
   const bool use_tc = ctx->denoiser_engine == 2 || (ctx->denoiser_engine == 0 && S >= kTcMinTokens);
-  if (use_tc) return enqueue_denoiser_tc(ctx, run, st);
+  if (use_tc) return enqueue_denoiser_tc(ctx, dev, run, st);
   const size_t need = sizeof(float) * denoiser_ws_floats(S);
   if (int rc = ensure_buffer(ctx, &ctx->den_ws, &ctx->den_ws_bytes, need)) return rc;
   float* ws = static_cast<float*>(ctx->den_ws);
@@ -187,53 +189,60 @@ int enqueue_denoiser(Context* ctx, DenoiserRun run, cudaStream_t st) {
   }
   if (flagged) {
     switch (TS) {
-      case 8: return launch_denoiser<8, true>(ctx, run, grid, st);
-      case 16: return launch_denoiser<16, true>(ctx, run, grid, st);
-      case 20: return launch_denoiser<20, true>(ctx, run, grid, st);
-      case 24: return launch_denoiser<24, true>(ctx, run, grid, st);
-      default: return launch_denoiser<32, true>(ctx, run, grid, st);
+      case 8: return launch_denoiser<8, true>(ctx, dev, run, grid, st);
+      case 16: return launch_denoiser<16, true>(ctx, dev, run, grid, st);
+      case 20: return launch_denoiser<20, true>(ctx, dev, run, grid, st);
+      case 24: return launch_denoiser<24, true>(ctx, dev, run, grid, st);
+      default: return launch_denoiser<32, true>(ctx, dev, run, grid, st);
     }
   }
   switch (TS) {
-    case 8: return launch_denoiser<8, false>(ctx, run, grid, st);
-    case 16: return launch_denoiser<16, false>(ctx, run, grid, st);
-    case 20: return launch_denoiser<20, false>(ctx, run, grid, st);
-    case 24: return launch_denoiser<24, false>(ctx, run, grid, st);
-    default: return launch_denoiser<32, false>(ctx, run, grid, st);
+    case 8: return launch_denoiser<8, false>(ctx, dev, run, grid, st);
+    case 16: return launch_denoiser<16, false>(ctx, dev, run, grid, st);
+    case 20: return launch_denoiser<20, false>(ctx, dev, run, grid, st);
+    case 24: return launch_denoiser<24, false>(ctx, dev, run, grid, st);
+    default: return launch_denoiser<32, false>(ctx, dev, run, grid, st);
   }
 }
 
 // The sampling loop in two halves, so that a caller can do host work (match packing) between them while the first half runs:
 // loop_prefix enqueues x_T = draws[0] (gaussian_diffuser.py:289) and the unguided steps t = T-1 .. guide_below in ONE launch,
-// loop_guided the guided steps (denoiser -> posterior mean -> GGS in place).
+// loop_guided the guided steps (denoiser -> posterior mean -> GGS in place).  A DDIM prefix (pdb_sample_loop_ddim) is k steps
+// on tables of virtual timesteps T-1 .. T-k; the guided steps that follow are the same DDPM steps either way.
 struct LoopState {
   DenoiserRun run = {};
   int guide_below = 0;
+  int prefix_steps = 0;  // unguided steps before the guided ones: T - guide_below (DDPM) or k (DDIM); trail slot of guided step i = 1 + prefix_steps + i
   bool first = true;
   size_t n = 0;
   float* pose = nullptr;
   float* trail = nullptr;
 };
 
+// ddim: NULL for the DDPM loop, else the k-step prefix's tables (make_ddim_tables) and noise_draws its draws (NULL: no noise).
 int loop_prefix(Context* ctx, const float* z_dev, const float* draws_dev, int batch, int frames, int guide_below, float* pose_dev,
-                float* trail_dev, cudaStream_t st, LoopState* loop) {
+                float* trail_dev, cudaStream_t st, LoopState* loop, const DenoiserDev* ddim = nullptr, int ddim_steps = 0,
+                const float* noise_draws = nullptr) {
   if (guide_below > kT) guide_below = kT;
   if (guide_below < 0) guide_below = 0;
+  const int prefix_steps = ddim ? ddim_steps : kT - guide_below;
   const size_t n = (size_t)batch * frames * kTargetDim;
   PDB_CUDA(ctx, cudaMemcpyAsync(pose_dev, draws_dev, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
   if (trail_dev) PDB_CUDA(ctx, cudaMemcpyAsync(trail_dev, draws_dev, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
   loop->n = n;
   loop->guide_below = guide_below;
+  loop->prefix_steps = prefix_steps;
   loop->pose = pose_dev;
   loop->trail = trail_dev;
   DenoiserRun& run = loop->run;
   run.batch = batch; run.frames = frames;
   run.guide_below = guide_below;
-  run.x = pose_dev; run.z = z_dev; run.draws = draws_dev; run.trail = trail_dev;
-  if (guide_below < kT) {
-    run.t_hi = kT - 1; run.t_lo = guide_below;
+  run.x = pose_dev; run.z = z_dev; run.draws = ddim ? noise_draws : draws_dev; run.trail = trail_dev;
+  if (prefix_steps > 0) {
+    // DDIM: virtual timesteps T-1 .. T-k, all >= guide_below, so the kernel adds noise (draw slot 1 + i) and writes trail slot 1 + i
+    run.t_hi = kT - 1; run.t_lo = kT - prefix_steps;
     run.compute_zproj = 1;
-    if (int rc = enqueue_denoiser(ctx, run, st)) return rc;
+    if (int rc = enqueue_denoiser(ctx, run, st, ddim)) return rc;
     loop->first = false;
   }
   return PDB_OK;
@@ -243,16 +252,100 @@ int loop_guided(Context* ctx, LoopState* loop, pdb_matches* const* problems, con
                 cudaStream_t st) {
   DenoiserRun& run = loop->run;
   for (int t = loop->guide_below - 1; t >= 0; --t) {
+    const int i = loop->guide_below - 1 - t;
     run.t_hi = run.t_lo = t;
     run.compute_zproj = loop->first ? 1 : 0;
     loop->first = false;
     if (int rc = enqueue_denoiser(ctx, run, st)) return rc;
-    pdb_ggs_stats* stats = stats_dev ? stats_dev + (size_t)(loop->guide_below - 1 - t) * run.batch : nullptr;
+    pdb_ggs_stats* stats = stats_dev ? stats_dev + (size_t)i * run.batch : nullptr;
     if (int rc = enqueue_ggs(ctx, problems, run.batch, run.frames, loop->pose, cfg, stats, st)) return rc;
     if (loop->trail)
-      PDB_CUDA(ctx, cudaMemcpyAsync(loop->trail + (size_t)(kT - t) * loop->n, loop->pose, sizeof(float) * loop->n,
+      PDB_CUDA(ctx, cudaMemcpyAsync(loop->trail + (size_t)(1 + loop->prefix_steps + i) * loop->n, loop->pose, sizeof(float) * loop->n,
                                     cudaMemcpyDeviceToDevice, st));
   }
+  return PDB_OK;
+}
+
+// float64 betas (torch.linspace: filled symmetrically from both ends) and their cumulative product
+void schedule_f64(double beta_1, double beta_T, double* beta, double* abar) {
+  const int n = kT;
+  const double step = (beta_T - beta_1) / (double)(n - 1);
+  for (int i = 0; i < n; ++i) beta[i] = (i < n / 2) ? beta_1 + step * i : beta_T - step * (n - 1 - i);
+  double prod = 1.0;
+  for (int i = 0; i < n; ++i) {
+    prod *= (1.0 - beta[i]);
+    abar[i] = prod;
+  }
+}
+
+// DDIM step table (Song et al. 2021, eq. 12; DESIGN.md "Fewer-step sampling").  Entries 0 .. k-1 (k = steps - guide_below) jump
+// tau_{k-i} -> tau_{k-i-1}, tau_j = (g - 1) + floor(j (T - g) / k), abar(-1) = 1; entries k .. steps-1 are the DDPM rows of the
+// guided timesteps g-1 .. 0.  False for k outside [1, T - g], eta < 0 or not finite, or an eta > 1 so large that
+// 1 - abar_s - sigma^2 < 0 at some jump.
+bool ddim_table(int steps, int guide_below, double eta, double beta_1, double beta_T, int32_t* t_out, float* coef_out) {
+  const int g = guide_below, k = steps - guide_below;
+  if (g < 0 || g > kT || k < 1 || k > kT - g || !std::isfinite(eta) || eta < 0.0) return false;
+  double beta[kT], abar[kT];
+  schedule_f64(beta_1, beta_T, beta, abar);
+  for (int i = 0; i < k; ++i) {
+    const int j = k - i;
+    const int t = (g - 1) + (int)((long long)j * (kT - g) / k);
+    const int s = (g - 1) + (int)((long long)(j - 1) * (kT - g) / k);
+    const double at = abar[t], as = s < 0 ? 1.0 : abar[s];
+    const double sigma = eta * std::sqrt((1.0 - as) / (1.0 - at)) * std::sqrt(1.0 - at / as);
+    const double rest = 1.0 - as - sigma * sigma;
+    if (!(rest >= 0.0)) return false;
+    const double c2 = std::sqrt(rest) / std::sqrt(1.0 - at);
+    const double c1 = std::sqrt(as) - c2 * std::sqrt(at);
+    float* r = coef_out + i * 8;
+    r[0] = (float)std::sqrt(1.0 / at);  // a_t, b_t exactly as the schedule rows hold them
+    r[1] = (float)std::sqrt(1.0 / at - 1.0);
+    r[2] = (float)c1;
+    r[3] = (float)c2;
+    r[4] = (float)sigma;
+    r[5] = (float)s;
+    r[6] = (float)at;
+    r[7] = (float)as;
+    t_out[i] = t;
+  }
+  float sched[kT * 8];
+  pdb_schedule_table(sched, beta_1, beta_T);
+  for (int i = 0; i < g; ++i) {
+    t_out[k + i] = g - 1 - i;
+    std::memcpy(coef_out + (size_t)(k + i) * 8, sched + (size_t)(g - 1 - i) * 8, sizeof(float) * 8);
+  }
+  return true;
+}
+
+// rows[kT - 1 - i] = src[t_i] (512 floats): the time-embedding block of step i's timestep at its virtual timestep
+struct RowMap { int src[kT]; };
+__global__ void gather_tproj_kernel(const float* __restrict__ src, float* __restrict__ dst, RowMap map) {
+  const int i = blockIdx.x;
+  for (int c = threadIdx.x; c < kDM; c += blockDim.x) dst[(size_t)(kT - 1 - i) * kDM + c] = src[(size_t)map.src[i] * kDM + c];
+}
+
+// The k-step DDIM prefix as the kernels see it: a copy of the weight descriptor whose per-timestep tables are indexed by the virtual
+// timestep v = T-1-i of prefix step i -- sched[v] = its DDIM coefficient row, tproj[v] = the time-embedding block of its real
+// timestep.  The DDPM loop over v = T-1 .. T-k then IS the DDIM prefix, draw and trail slot 1 + i included.  The tables live in a
+// context-owned buffer at a fixed address, rewritten (stream-ordered) before each loop.
+int make_ddim_tables(Context* ctx, const int32_t* tab_t, const float* tab_coef, int k, cudaStream_t st, DenoiserDev* out) {
+  const size_t sched_floats = (size_t)kT * 8, bytes = sizeof(float) * (sched_floats + (size_t)kT * kDM);
+  if (!ctx->step_tab) PDB_CUDA(ctx, cudaMalloc(&ctx->step_tab, bytes));
+  float* vsched = static_cast<float*>(ctx->step_tab);
+  float* vtproj = vsched + sched_floats;
+  float rows[kT * 8] = {};
+  RowMap map = {};
+  for (int i = 0; i < k; ++i) {
+    std::memcpy(rows + (size_t)(kT - 1 - i) * 8, tab_coef + (size_t)i * 8, sizeof(float) * 8);
+    map.src[i] = tab_t[i];
+  }
+  PDB_CUDA(ctx, cudaMemcpyAsync(vsched, rows, sizeof(rows), cudaMemcpyHostToDevice, st));
+  *out = ctx->weights->dev;
+  gather_tproj_kernel<<<k, 128, 0, st>>>(out->tproj, vtproj, map);
+  PDB_CUDA(ctx, cudaGetLastError());
+  ctx->launches += 1;
+  out->tproj = vtproj;
+  out->sched = vsched;
   return PDB_OK;
 }
 
@@ -274,6 +367,7 @@ void pdb_destroy(pdb_context* c) {
   if (ctx->ggs_ws) cudaFree(ctx->ggs_ws);
   if (ctx->den_ws) cudaFree(ctx->den_ws);
   if (ctx->den_flag_ws) cudaFree(ctx->den_flag_ws);
+  if (ctx->step_tab) cudaFree(ctx->step_tab);
   if (ctx->stage) cudaFree(ctx->stage);
   if (ctx->tc_graph) cudaGraphExecDestroy(ctx->tc_graph);
   if (ctx->tc_capture_stream) cudaStreamDestroy(ctx->tc_capture_stream);
@@ -297,14 +391,7 @@ int pdb_schedule_table(float* out, double beta_1, double beta_T) {
   if (!out) return PDB_ERR_INVALID;
   const int n = kT;
   double beta[kT], abar[kT];
-  const double step = (beta_T - beta_1) / (double)(n - 1);
-  for (int i = 0; i < n; ++i)  // torch.linspace fills symmetrically from both ends
-    beta[i] = (i < n / 2) ? beta_1 + step * i : beta_T - step * (n - 1 - i);
-  double prod = 1.0;
-  for (int i = 0; i < n; ++i) {
-    prod *= (1.0 - beta[i]);
-    abar[i] = prod;
-  }
+  schedule_f64(beta_1, beta_T, beta, abar);
   for (int i = 0; i < n; ++i) {
     const double prev = i ? abar[i - 1] : 1.0;
     const double pv = beta[i] * (1.0 - prev) / (1.0 - abar[i]);
@@ -550,6 +637,43 @@ int pdb_sample_loop(pdb_context* c, const float* z_dev, const float* draws_dev, 
   PDB_CUDA(ctx, cudaSetDevice(ctx->device));
   LoopState loop;
   if (int rc = loop_prefix(ctx, z_dev, draws_dev, batch, frames, problems ? cond_start_step : 0, pose_dev, trail_dev, st, &loop)) return rc;
+  return loop_guided(ctx, &loop, problems, cfg, stats_dev, st);
+}
+
+int pdb_ddim_table(int32_t steps, int32_t guide_below, double eta, double beta_1, double beta_T, int32_t* t_out, float* coef_out) {
+  if (!t_out || !coef_out) return PDB_ERR_INVALID;
+  return ddim_table(steps, guide_below, eta, beta_1, beta_T, t_out, coef_out) ? PDB_OK : PDB_ERR_INVALID;
+}
+
+int pdb_sample_loop_ddim(pdb_context* c, const float* z_dev, const float* draws_dev, int32_t batch, int32_t frames, int32_t steps,
+                         double eta, pdb_matches* const* problems, int32_t n_problems, const pdb_ggs_config* cfg, int32_t cond_start_step,
+                         float* pose_dev, float* trail_dev, pdb_ggs_stats* stats_dev, void* stream) {
+  if (!c) return PDB_ERR_INVALID;
+  Context* ctx = reinterpret_cast<Context*>(c);
+  if (!z_dev || !draws_dev || !pose_dev) return ctx->fail(PDB_ERR_INVALID, "null argument");
+  if (batch < 1 || frames < 1) return ctx->fail(PDB_ERR_INVALID, "empty batch");
+  if (frames > PDB_MAX_FRAMES) return ctx->fail(PDB_ERR_LIMIT, "frames %d > PDB_MAX_FRAMES", frames);
+  if (problems && !cfg) return ctx->fail(PDB_ERR_INVALID, "GGS config missing");
+  if (problems && n_problems != batch)
+    return ctx->fail(PDB_ERR_INVALID, "%d match sets for a batch of %d sequences (one per sequence)", n_problems, batch);
+  const int g = cond_start_step < 0 ? 0 : (cond_start_step > kT ? kT : cond_start_step);
+  int32_t tab_t[kT];
+  float tab_coef[kT * 8];
+  if (!ddim_table(steps, g, eta, 1e-4, 0.1, tab_t, tab_coef))
+    return ctx->fail(PDB_ERR_INVALID, "DDIM: %d denoiser steps with %d guided (the unguided prefix needs 1 .. %d) and eta %g (>= 0, finite)",
+                     steps, g, kT - g, eta);
+  if (problems)
+    if (int rc = check_ggs_problems(ctx, problems, batch, frames)) return rc;
+  if (!ctx->weights) return ctx->fail(PDB_ERR_STATE, "denoiser weights not loaded (pdb_denoiser_load)");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  PDB_CUDA(ctx, cudaSetDevice(ctx->device));
+  DenoiserDev tables;
+  if (int rc = make_ddim_tables(ctx, tab_t, tab_coef, steps - g, st, &tables)) return rc;
+  LoopState loop;
+  if (int rc = loop_prefix(ctx, z_dev, draws_dev, batch, frames, g, pose_dev, trail_dev, st, &loop, &tables, steps - g,
+                           eta > 0.0 ? draws_dev : nullptr))
+    return rc;
+  if (!problems) return PDB_OK;  // cond_start_step > 0 without match sets: the prefix alone, x_{g-1} (generic cond_fn callers)
   return loop_guided(ctx, &loop, problems, cfg, stats_dev, st);
 }
 

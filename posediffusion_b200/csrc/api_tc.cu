@@ -278,7 +278,8 @@ __global__ void step_dec_kernel(int* tstate) {
 
 namespace pdb {
 
-int enqueue_denoiser_tc(Context* ctx, DenoiserRun run, cudaStream_t st) {
+// `dev` is the loaded weights' descriptor, or its copy with a DDIM prefix's per-timestep tables (tproj, sched; api_sampler.cu).
+int enqueue_denoiser_tc(Context* ctx, const DenoiserDev& dev, DenoiserRun run, cudaStream_t st) {
   const DenoiserWeights* w = ctx->weights;
   const TcWeights& T = w->tc;
   const int S = run.tokens, B = run.batch, N = run.frames;
@@ -330,7 +331,7 @@ int enqueue_denoiser_tc(Context* ctx, DenoiserRun run, cudaStream_t st) {
     // gain from overlapping a kernel's prologue with its predecessor's tail
     pdl = ctx->tc_pdl && S <= 320;
     PDB_CUDA(ctx, launch_chained(embed_kernel, dim3((S * kPoseEmbPad + 255) / 256), dim3(256), 0, s, false, (const float*)run.x, emb, S));
-    if (int rc = lin(emb, T.wx, kDM, kPoseEmbPad, T.tproj, tstate, run.zproj, kDM, nullptr, run.h, 0, s)) return rc;
+    if (int rc = lin(emb, T.wx, kDM, kPoseEmbPad, dev.tproj, tstate, run.zproj, kDM, nullptr, run.h, 0, s)) return rc;
     for (int l = 0; l < kLayers; ++l) {
       const TcLayer& L = T.layer[l];
       if (!stats_qkv) PDB_CUDA(ctx, launch_chained(row_stats_kernel, dim3((S + 7) / 8), dim3(256), 0, s, pdl, (const float*)run.h, mean, rstd, S));
@@ -342,7 +343,7 @@ int enqueue_denoiser_tc(Context* ctx, DenoiserRun run, cudaStream_t st) {
       if (int rc = lin(run.ff, L.wff2, kDM, kFF, L.bff2, nullptr, run.h, kDM, nullptr, run.h, 0, s)) return rc;
     }
     if (int rc = lin(run.h, T.wlast0, kHid, kDM, T.blast0, nullptr, nullptr, 0, nullptr, run.u, 0, s)) return rc;
-    PDB_CUDA(ctx, launch_chained(tail_kernel, dim3((S + kDenWarps - 1) / kDenWarps), dim3(kDenThreads), 0, s, pdl, w->dev, run, (const int*)tstate));
+    PDB_CUDA(ctx, launch_chained(tail_kernel, dim3((S + kDenWarps - 1) / kDenWarps), dim3(kDenThreads), 0, s, pdl, dev, run, (const int*)tstate));
     PDB_CUDA(ctx, launch_chained(step_dec_kernel, dim3(1), dim3(1), 0, s, pdl, tstate));
     pdl = false;
     return PDB_OK;
@@ -350,7 +351,7 @@ int enqueue_denoiser_tc(Context* ctx, DenoiserRun run, cudaStream_t st) {
   const int kNodes = 2 + kLayers * (7 - (stats_qkv ? 1 : 0) - (stats_ff1 ? 1 : 0)) + 3;
   std::vector<size_t> key = {(size_t)S, (size_t)B, (size_t)N, (size_t)run.guide_below, (size_t)ctx->den_ws, (size_t)run.x,
                              (size_t)run.draws, (size_t)run.trail, (size_t)run.eps_out, (size_t)run.x0_out, (size_t)run.mean_out,
-                             (size_t)w->tc_arena, (size_t)ctx->tc_swap, (size_t)stats_qkv, (size_t)stats_ff1,
+                             (size_t)w->tc_arena, (size_t)dev.tproj, (size_t)dev.sched, (size_t)ctx->tc_swap, (size_t)stats_qkv, (size_t)stats_ff1,
                              (size_t)tc_linear_small(ctx, S, kDM), (size_t)(ctx->tc_pdl && S <= 320)};  // launcher regime: the captured kernels differ
   if (!ctx->tc_graph || ctx->tc_graph_key != key) {
     if (ctx->tc_graph) { cudaGraphExecDestroy(ctx->tc_graph); ctx->tc_graph = nullptr; }

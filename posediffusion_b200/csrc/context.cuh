@@ -35,6 +35,9 @@ struct Context {
   void* den_flag_ws = nullptr;
   size_t den_flag_ws_bytes = 0;
   unsigned den_tag = 1;  // next unused version tag (0 = never written)
+  // per-timestep tables of the current DDIM prefix (pdb_sample_loop_ddim): sched [100][8], then tproj [100][512], indexed by
+  // virtual timestep.  Allocated once, so its address never changes; rewritten, stream-ordered, before each loop.
+  void* step_tab = nullptr;
   // stage timing probe of the GGS kernel (debug): [ctas][8] cycle sums
   long long* ggs_clock = nullptr;
   int ggs_clock_ctas = 0;

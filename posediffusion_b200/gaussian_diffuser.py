@@ -8,6 +8,10 @@ denoiser + GGS launches per guided step) when `cond_fn` is None or a `partial(ge
 of this package; any other callable falls back to a Python loop around the native single-step kernel --
 still CUDA-only.  Gaussian draws come from torch's generator on the sampler's device in the reference's
 order (one `randn(shape)` then one `randn_like` per unguided step with t > 0, :289, :278).
+
+`ddim_sample` is the fewer-step sampling the reference's `sampling_timesteps` argument names but never built (:79, :150-154,
+:303-306): the unguided prefix in k < 100 DDIM steps (Song et al. 2021, eq. 12), then exactly `p_sample_loop`'s guided tail.
+`sample` / `p_sample_loop` do not change: DDIM is opt-in.
 """
 from __future__ import annotations
 
@@ -117,10 +121,7 @@ class GaussianDiffusion(nn.Module):
         device = self.betas.device
         ctx = self.model.native_context()
         z = z.contiguous().float()
-        fused = cond_fn is None or (
-            isinstance(cond_fn, partial) and cond_fn.func is geometry_guided_sampling and not cond_fn.args
-            and set(cond_fn.keywords) == {"matches_dict", "GGS_cfg"}
-        )
+        fused = self._fused(cond_fn)
         guided_below = cond_start_step if cond_fn is not None else 0
         if draws is None:
             draws = self.draw_noise(tuple(shape), device, guided_below)
@@ -147,6 +148,61 @@ class GaussianDiffusion(nn.Module):
             pose = cond_fn(mean, t) if guided else pred
             trail.append(pose.unsqueeze(0))
         return pose, torch.cat(trail)
+
+    def _fused(self, cond_fn) -> bool:
+        return cond_fn is None or (
+            isinstance(cond_fn, partial) and cond_fn.func is geometry_guided_sampling and not cond_fn.args
+            and set(cond_fn.keywords) == {"matches_dict", "GGS_cfg"}
+        )
+
+    def ddim_draws(self, shape, device, k: int, eta: float) -> torch.Tensor:
+        """Gaussian draws of `ddim_sample` on `device`'s generator: one `randn(shape)` for x_T, then, when eta > 0, one per unguided
+        DDIM step ([1 + k, B, N, 9]; k = steps minus the guided steps, which add no noise); [1, B, N, 9] when eta == 0."""
+        draws = [torch.randn(shape, device=device)]
+        if eta > 0:
+            draws += [torch.randn(shape, device=device) for _ in range(k)]
+        return torch.stack(draws)
+
+    @torch.no_grad()
+    def ddim_sample(self, shape, z: torch.Tensor, cond_fn: Optional[Callable] = None, cond_start_step: int = 0,
+                    sampling_timesteps: Optional[int] = None, eta: float = 0.0, draws: Optional[torch.Tensor] = None):
+        """(pose [B,N,9], trail [1 + k + g, B, N, 9]) in `sampling_timesteps` denoiser evaluations (default: the constructor's
+        `sampling_timesteps`).  g = clamp(cond_start_step, 0, 100) guided steps when cond_fn is given (else 0) run exactly as in
+        `p_sample_loop`; the k = sampling_timesteps - g unguided ones are DDIM jumps with noise scale eta (0: deterministic, 1: the
+        DDPM posterior variance; at k = 100 - g and eta = 1 the steps are DDPM's).  k and eta trade speed against sample quality;
+        the released checkpoint's pose accuracy under DDIM has not been measured.  ValueError for k outside [1, 100 - g] or an eta
+        that is negative or not finite.  `draws` as `ddim_draws` makes them."""
+        self._require_native()
+        steps = self.sampling_timesteps if sampling_timesteps is None else int(sampling_timesteps)
+        guided = max(0, min(int(cond_start_step), self.num_timesteps)) if cond_fn is not None else 0
+        eta = float(eta)
+        k = _native.ddim_check(steps, guided, eta)
+        device = self.betas.device
+        ctx = self.model.native_context()
+        z = z.contiguous().float()
+        if draws is None:
+            draws = self.ddim_draws(tuple(shape), device, k, eta)
+        draws = draws.contiguous()
+        if self._fused(cond_fn):
+            problems = cfg = None
+            if cond_fn is not None:
+                cfg = cond_fn.keywords["GGS_cfg"]
+                problems = packed_matches(ctx, cond_fn.keywords["matches_dict"])
+            pose, trail, stats = ctx.sample_loop_ddim(z, draws, steps, eta, problems, cfg, guided)
+            self.last_ggs_stats = stats
+            if stats is not None and bool(cfg.get("verbose", True)):
+                rows = _native.stats_to_numpy(stats).reshape(-1, shape[0])
+                for i, per_step in enumerate(rows):
+                    for row in per_step:
+                        print("\n".join(format_log(guided - 1 - i, row)))
+            return pose, trail
+        # generic cond_fn: the DDIM prefix natively (it stops at x_{g-1}), then the guided DDPM steps around the native step
+        pose, trail, _ = ctx.sample_loop_ddim(z, draws, steps, eta, None, None, guided)
+        for i, t in enumerate(reversed(range(guided))):
+            _, mean, _ = ctx.p_sample(pose, t, z, None)
+            pose = cond_fn(mean, t)
+            trail[1 + k + i] = pose
+        return pose, trail
 
     @torch.no_grad()
     def sample(self, shape, z, cond_fn=None, cond_start_step=0):

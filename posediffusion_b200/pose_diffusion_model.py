@@ -58,7 +58,8 @@ class PoseDiffusionModel(nn.Module):
             nn.init.constant_(m.weight, 1.0)
 
     def forward(self, image: Optional[torch.Tensor] = None, gt_cameras=None, sequence_name: Optional[List[str]] = None,
-                cond_fn=None, cond_start_step=0, training=True, batch_repeat=-1, z: Optional[torch.Tensor] = None):
+                cond_fn=None, cond_start_step=0, training=True, batch_repeat=-1, z: Optional[torch.Tensor] = None,
+                sampling_timesteps: Optional[int] = None, eta: float = 0.0):
         if z is None:
             if self.image_feature_extractor is None or image is None:
                 raise ValueError("no image feature extractor configured: pass precomputed features as z=[B,N,384]")
@@ -87,8 +88,14 @@ class PoseDiffusionModel(nn.Module):
             )
             return diffusion_results
         B, N, _ = z.shape
-        pose_encoding, _trajectory = self.diffuser.sample(
-            shape=[B, N, self.target_dim], z=z, cond_fn=cond_fn, cond_start_step=cond_start_step
-        )
+        if sampling_timesteps is None:
+            pose_encoding, _trajectory = self.diffuser.sample(
+                shape=[B, N, self.target_dim], z=z, cond_fn=cond_fn, cond_start_step=cond_start_step
+            )
+        else:  # fewer denoiser steps: DDIM over the unguided prefix (GaussianDiffusion.ddim_sample)
+            pose_encoding, _trajectory = self.diffuser.ddim_sample(
+                shape=[B, N, self.target_dim], z=z, cond_fn=cond_fn, cond_start_step=cond_start_step,
+                sampling_timesteps=sampling_timesteps, eta=eta
+            )
         pred_cameras = pose_encoding_to_camera(pose_encoding, pose_encoding_type=self.pose_encoding_type)
         return {"pred_cameras": pred_cameras, "z": z}
