@@ -18,10 +18,13 @@
  *   pdb_sample_loop        <- GaussianDiffusion.sample / p_sample_loop   (models/gaussian_diffuser.py:285-306)
  *   pdb_sample_loop_ddim   <- the fewer-step sampling the reference's `sampling_timesteps` names but never built (:79, :150-154,
  *                             :303-306): a DDIM prefix in k < 100 steps, then the same guided DDPM + GGS tail
+ *   pdb_sample_loop_ddim_guided <- the same with the guided tail in g' < g DDIM jumps, GGS after each (no reference
+ *                             counterpart: the reference's guided steps are always the g DDPM steps)
  *   pdb_sample_loop_host   <- the same call with HOST buffers (demo.py:108 as a user sees it: features and
  *                             matches on the host, poses back on the host)
  *   pdb_sample_loop_host_matches <- the same call starting from the reference's matches_dict arrays (demo.py:94-108:
  *                             extract_match output straight into the sampler); packing overlaps the unguided steps
+ *   pdb_sample_loop_host_matches_ddim <- that call on the loop of pdb_sample_loop_ddim_guided
  *   pdb_images_preprocess_host <- load_and_preprocess_images after PIL decoding (util/load_img_folder.py: float conversion,
  *                             centre crop, bilinear resize; demo.py:51, test.py:172)
  *
@@ -135,8 +138,16 @@ int pdb_schedule_table(float* out, double beta_1, double beta_T);
  * abar_t/abar_s), c2 = sqrt(1 - abar_s - sigma^2) / sqrt(1 - abar_t), c1 = sqrt(abar_s) - c2 sqrt(abar_t), abar_{-1} = 1; entries
  * k .. steps-1 are the pdb_schedule_table rows of timesteps g-1 .. 0 (the guided tail stays DDPM).  With k = 100 - g and eta = 1
  * the prefix rows equal the DDPM posterior rows up to rounding.  PDB_ERR_INVALID for k out of range, eta < 0 or not finite, or
- * an eta > 1 large enough to make 1 - abar_s - sigma^2 negative. */
+ * an eta > 1 large enough to make 1 - abar_s - sigma^2 negative.  It is pdb_ddim_table_guided with guided_steps = guide_below. */
 int pdb_ddim_table(int32_t steps, int32_t guide_below, double eta, double beta_1, double beta_T, int32_t* t_out, float* coef_out);
+
+/* pdb_ddim_table with the guided tail in g' = `guided_steps` denoiser evaluations, 1 <= g' <= g (g' = 0 when g = 0): the prefix
+ * takes k = steps - g' steps (still 1 <= k <= 100 - g).  With g' == g entries k .. steps-1 are the DDPM rows, exactly as
+ * pdb_ddim_table writes them; with g' < g they are g' DDIM jumps of the same form and eta as the prefix's, entry k + i jumping
+ * tau'_{g'-i} -> tau'_{g'-i-1}, tau'_j = floor(j * g / g') - 1 (tau'_{g'} = g - 1, tau'_0 = -1 = x0).  The samplers add no noise
+ * on guided jumps (sigma is tabulated all the same).  HOST-ONLY; PDB_ERR_INVALID as pdb_ddim_table, and for g' out of range. */
+int pdb_ddim_table_guided(int32_t steps, int32_t guide_below, int32_t guided_steps, double eta, double beta_1, double beta_T,
+                          int32_t* t_out, float* coef_out);
 
 /* ---- denoiser weights ---------------------------------------------------------------------------
  * `tensors[i]` (host or device, fp32, contiguous) in the order of the reference state_dict below
@@ -223,10 +234,20 @@ int pdb_sample_loop(pdb_context* ctx, const float* z_dev, const float* draws_dev
  * with cond_start_step > 0 runs the prefix alone and leaves x_{g-1} in pose_dev (a caller's own guidance takes over from there).
  * PDB_ERR_INVALID before anything is enqueued for k out of range, a bad eta or a NULL draws pointer; PDB_ERR_LIMIT for frames >
  * PDB_MAX_FRAMES.  The step table is copied (stream-ordered) into a buffer the context owns; concurrent loops on one context
- * must share a stream. */
+ * must share a stream.  It is pdb_sample_loop_ddim_guided with guided_steps = g. */
 int pdb_sample_loop_ddim(pdb_context* ctx, const float* z_dev, const float* draws_dev, int32_t batch, int32_t frames, int32_t steps,
                          double eta, pdb_matches* const* problems, int32_t n_problems, const pdb_ggs_config* cfg,
                          int32_t cond_start_step, float* pose_dev, float* trail_dev, pdb_ggs_stats* stats_dev, void* stream);
+
+/* pdb_sample_loop_ddim with the guided tail in g' = `guided_steps` jumps (pdb_ddim_table_guided): k = steps - g' prefix steps,
+ * then per jump one denoiser step to the DDIM mean (no noise, no draw) and GGS on it in place, with the same cfg (its iteration
+ * counts are not rescaled by the stride).  g' == g is exactly pdb_sample_loop_ddim.  trail_dev [1 + k + g', B, N, 9], stats_dev
+ * [g', batch] records.  PDB_ERR_INVALID before anything is enqueued for g' outside [1, g] (0 when g = 0), k outside [1, 100 - g]
+ * or a bad eta. */
+int pdb_sample_loop_ddim_guided(pdb_context* ctx, const float* z_dev, const float* draws_dev, int32_t batch, int32_t frames,
+                                int32_t steps, double eta, int32_t guided_steps, pdb_matches* const* problems, int32_t n_problems,
+                                const pdb_ggs_config* cfg, int32_t cond_start_step, float* pose_dev, float* trail_dev,
+                                pdb_ggs_stats* stats_dev, void* stream);
 
 /* The same with host buffers (pinned or pageable): copies z and the draws in, runs, copies pose (and the
  * optional trajectory / stats) out, synchronises the stream.  This is the end-to-end call bench.py times. */
@@ -245,6 +266,15 @@ int pdb_sample_loop_host_matches(pdb_context* ctx, const float* z_host, const fl
                                  const int64_t* m_total, int32_t height, int32_t width, const pdb_ggs_config* cfg,
                                  int32_t cond_start_step, float* pose_host, float* trail_host, pdb_ggs_stats* stats_host,
                                  void* stream);
+
+/* pdb_sample_loop_host_matches on the loop of pdb_sample_loop_ddim_guided: the sets are packed while the DDIM prefix runs.
+ * draws_host [1 + k, B, N, 9] for eta > 0, [1, B, N, 9] for eta == 0; trail_host [1 + k + g', B, N, 9]; stats_host [g', batch].
+ * The same refusals as pdb_sample_loop_ddim_guided, before anything is enqueued. */
+int pdb_sample_loop_host_matches_ddim(pdb_context* ctx, const float* z_host, const float* draws_host, int32_t batch, int32_t frames,
+                                      int32_t steps, double eta, int32_t guided_steps, const double* const* kp1,
+                                      const double* const* kp2, const int64_t* const* i12, const int64_t* m_total, int32_t height,
+                                      int32_t width, const pdb_ggs_config* cfg, int32_t cond_start_step, float* pose_host,
+                                      float* trail_host, pdb_ggs_stats* stats_host, void* stream);
 
 /* ---- image features (widened row, SURVEY 8f-2) ---------------------------------------------------
  * z = MultiScaleImageFeatureExtractor(image) (models/image_feature_extractor.py:27-87): the DINO ViT-S/16 backbone that the

@@ -75,6 +75,14 @@ EXPORTS = {
     "pdb_ddim_table": (C.c_int, [C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_void_p, C.c_void_p]),
     "pdb_sample_loop_ddim": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.POINTER(C.c_void_p),
                                        C.c_int32, C.POINTER(GgsConfig), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pdb_ddim_table_guided": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_void_p, C.c_void_p]),
+    "pdb_sample_loop_ddim_guided": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_int32,
+                                              C.POINTER(C.c_void_p), C.c_int32, C.POINTER(GgsConfig), C.c_int32, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p]),
+    "pdb_sample_loop_host_matches_ddim": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_int32,
+                                                    C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int64),
+                                                    C.c_int32, C.c_int32, C.POINTER(GgsConfig), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                    C.c_void_p]),
     "pdb_denoiser_load": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_int32, C.c_void_p]),
     "pdb_denoiser_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "pdb_p_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -179,25 +187,42 @@ def schedule_table(beta_1: float = 1e-4, beta_T: float = 0.1) -> np.ndarray:
     return out
 
 
-def ddim_table(steps: int, guide_below: int = 0, eta: float = 0.0, beta_1: float = 1e-4, beta_T: float = 0.1):
-    """(t [steps] int32, coef [steps, 8] float32): the DDIM step table of pdb_ddim_table -- `steps` denoiser evaluations, the last
-    `guide_below` of them guided DDPM steps (no GPU needed).  ValueError where the library refuses the arguments."""
+def ddim_table(steps: int, guide_below: int = 0, eta: float = 0.0, beta_1: float = 1e-4, beta_T: float = 0.1,
+               guided_steps: Optional[int] = None):
+    """(t [steps] int32, coef [steps, 8] float32): the DDIM step table of pdb_ddim_table_guided -- `steps` denoiser evaluations,
+    the last g' = `guided_steps` (default `guide_below`) of them the guided tail over timesteps guide_below-1 .. 0: DDPM rows when
+    g' = guide_below, DDIM jumps when g' is smaller (no GPU needed).  ValueError where the library refuses the arguments."""
+    gs = int(guide_below) if guided_steps is None else int(guided_steps)
     n = max(int(steps), 1)
     t = np.zeros(n, dtype=np.int32)
     coef = np.zeros((n, 8), dtype=np.float32)
-    rc = load_library().pdb_ddim_table(int(steps), int(guide_below), float(eta), beta_1, beta_T, t.ctypes.data_as(C.c_void_p),
-                                       coef.ctypes.data_as(C.c_void_p))
+    rc = load_library().pdb_ddim_table_guided(int(steps), int(guide_below), gs, float(eta), beta_1, beta_T,
+                                              t.ctypes.data_as(C.c_void_p), coef.ctypes.data_as(C.c_void_p))
     if rc != 0:
-        raise ValueError(f"pdb_ddim_table refused steps={steps}, guide_below={guide_below}, eta={eta}")
+        raise ValueError(f"pdb_ddim_table_guided refused steps={steps}, guide_below={guide_below}, guided_steps={gs}, eta={eta}")
     return t, coef
 
 
-def ddim_check(steps: int, guided: int, eta: float) -> int:
-    """k = steps - guided unguided DDIM steps, or ValueError (the library's own check, mirrored so that nothing is enqueued)."""
-    k = int(steps) - int(guided)
-    if not 1 <= k <= NUM_TIMESTEPS - int(guided):
-        raise ValueError(f"sampling_timesteps={steps} with {guided} guided steps leaves {k} unguided DDIM steps; "
-                         f"1 .. {NUM_TIMESTEPS - int(guided)} are possible")
+def guided_times(g: int, guided_steps: int) -> List[int]:
+    """tau'_0 .. tau'_{g'} = floor(j g / g') - 1 of the g' guided jumps over timesteps g-1 .. 0 (pdb_ddim_table_guided); jump i
+    runs the network at tau'_{g'-i}."""
+    return [(j * int(g)) // int(guided_steps) - 1 for j in range(int(guided_steps) + 1)]
+
+
+def ddim_check(steps: int, guided: int, eta: float, guided_steps: Optional[int] = None) -> int:
+    """k = steps - g' unguided DDIM steps (g' = `guided_steps`, default `guided`), or ValueError (the library's own check, mirrored
+    so that nothing is enqueued)."""
+    g = int(guided)
+    if guided_steps is not None:
+        if g == 0:
+            raise ValueError(f"guided_steps={guided_steps} without guidance (no cond_fn, or cond_start_step 0)")
+        if not 1 <= int(guided_steps) <= g:
+            raise ValueError(f"guided_steps={guided_steps}: the {g} guided timesteps take 1 .. {g} denoiser steps")
+    gs = g if guided_steps is None else int(guided_steps)
+    k = int(steps) - gs
+    if not 1 <= k <= NUM_TIMESTEPS - g:
+        raise ValueError(f"sampling_timesteps={steps} with {gs} guided steps leaves {k} unguided DDIM steps; "
+                         f"1 .. {NUM_TIMESTEPS - g} are possible")
     if not math.isfinite(float(eta)) or float(eta) < 0.0:
         raise ValueError(f"eta={eta}: DDIM needs a finite eta >= 0")
     return k
@@ -702,28 +727,32 @@ class Context:
         return pose, trail, stats
 
     def sample_loop_ddim(self, z: torch.Tensor, draws: torch.Tensor, steps: int, eta: float, problems: Optional[Sequence[Matches]],
-                         cfg: Optional[Dict], cond_start_step: int, want_trail: bool = True, want_stats: bool = True):
-        """pdb_sample_loop_ddim: (pose, trail [1 + steps, B, N, 9] or None, stats).  draws [1 + k, B, N, 9] for eta > 0, [1, B, N, 9]
-        for eta == 0 (k = steps - guided).  Without problems and with cond_start_step > 0 only the prefix runs (pose = x_{g-1})."""
+                         cfg: Optional[Dict], cond_start_step: int, want_trail: bool = True, want_stats: bool = True,
+                         guided_steps: Optional[int] = None):
+        """pdb_sample_loop_ddim_guided: (pose, trail [1 + steps, B, N, 9] or None, stats [g', B] records).  The guided tail over
+        g = clamp(cond_start_step) timesteps takes g' = `guided_steps` (default g) jumps, the prefix k = steps - g'.  draws
+        [1 + k, B, N, 9] for eta > 0, [1, B, N, 9] for eta == 0.  Without problems and with cond_start_step > 0 only the prefix runs
+        (pose = x_{g-1})."""
         B, N, _ = z.shape
         _check_dev(z, "z", self.device, (B, N, Z_DIM))
         guided = max(0, min(int(cond_start_step), NUM_TIMESTEPS))
-        k = ddim_check(steps, guided, eta)
+        k = ddim_check(steps, guided, eta, guided_steps)
+        gs = guided if guided_steps is None else int(guided_steps)
         _check_dev(draws, "draws", self.device, (1 + k if eta > 0 else 1, B, N, TARGET_DIM))
         if problems:
             self._check_problems(problems, B, N)
         pose = torch.empty(B, N, TARGET_DIM, device=self.device)
         trail = torch.empty(1 + int(steps), B, N, TARGET_DIM, device=self.device) if want_trail else None
         stats = None
-        if want_stats and problems and guided:
-            stats = torch.zeros(guided * B * GGS_STATS_DTYPE.itemsize, dtype=torch.uint8, device=self.device)
+        if want_stats and problems and gs:
+            stats = torch.zeros(gs * B * GGS_STATS_DTYPE.itemsize, dtype=torch.uint8, device=self.device)
         conf = ggs_config_struct(cfg) if problems else None
-        self._ok(self.lib.pdb_sample_loop_ddim(self.handle, z.data_ptr(), draws.data_ptr(), B, N, int(steps), float(eta),
-                                               self._problem_array(problems) if problems else None, len(problems) if problems else 0,
-                                               C.byref(conf) if conf is not None else None, int(cond_start_step), pose.data_ptr(),
-                                               trail.data_ptr() if want_trail else None,
-                                               stats.data_ptr() if stats is not None else None, _stream_ptr(self.device)),
-                 "pdb_sample_loop_ddim")
+        self._ok(self.lib.pdb_sample_loop_ddim_guided(self.handle, z.data_ptr(), draws.data_ptr(), B, N, int(steps), float(eta), gs,
+                                                      self._problem_array(problems) if problems else None,
+                                                      len(problems) if problems else 0, C.byref(conf) if conf is not None else None,
+                                                      int(cond_start_step), pose.data_ptr(), trail.data_ptr() if want_trail else None,
+                                                      stats.data_ptr() if stats is not None else None, _stream_ptr(self.device)),
+                 "pdb_sample_loop_ddim_guided")
         return pose, trail, stats
 
     def sample_loop_host(self, z: np.ndarray, draws: np.ndarray, problems, cfg, cond_start_step: int,
@@ -748,6 +777,51 @@ class Context:
         """The end-to-end call from the reference's matches_dict format (one dict per sequence): the match sets are packed and
         uploaded while the unguided steps already run (pdb_sample_loop_host_matches)."""
         B, N, _ = z.shape
+        ptrs, counts, shape, _keep = self._host_match_arrays(matches_dicts, B, N)
+        conf = ggs_config_struct(cfg)
+        with torch.cuda.device(self.device):
+            rc = self.lib.pdb_sample_loop_host_matches(self.handle, z.ctypes.data, draws.ctypes.data, B, N, ptrs[0], ptrs[1], ptrs[2],
+                                                       counts, shape[0], shape[1], C.byref(conf), int(cond_start_step),
+                                                       pose_out.ctypes.data, trail_out.ctypes.data if trail_out is not None else None,
+                                                       stats_out.ctypes.data if stats_out is not None else None,
+                                                       _stream_ptr(self.device))
+        if rc == -1:
+            raise ValueError(self.lib.pdb_last_error(self.handle).decode())
+        self._ok(rc, "pdb_sample_loop_host_matches")
+        return pose_out
+
+    def sample_loop_host_matches_ddim(self, z: np.ndarray, draws: np.ndarray, matches_dicts, cfg, cond_start_step: int, steps: int,
+                                      eta: float, pose_out: np.ndarray, trail_out: Optional[np.ndarray] = None,
+                                      stats_out: Optional[np.ndarray] = None, guided_steps: Optional[int] = None):
+        """sample_loop_host_matches on the DDIM loop of sample_loop_ddim (pdb_sample_loop_host_matches_ddim): draws [1 + k, B, N, 9]
+        for eta > 0, [1, B, N, 9] for eta == 0; trail_out [1 + steps, B, N, 9]; stats_out g' records per sequence."""
+        B, N, _ = z.shape
+        guided = max(0, min(int(cond_start_step), NUM_TIMESTEPS))
+        k = ddim_check(steps, guided, eta, guided_steps)
+        gs = guided if guided_steps is None else int(guided_steps)
+        if draws.shape != (1 + k if eta > 0 else 1, B, N, TARGET_DIM) or draws.dtype != np.float32 or not draws.flags.c_contiguous:
+            raise ValueError(f"draws must be C-contiguous float32 {(1 + k if eta > 0 else 1, B, N, TARGET_DIM)}, got {draws.shape}")
+        if trail_out is not None and trail_out.shape != (1 + int(steps), B, N, TARGET_DIM):
+            raise ValueError(f"trail_out must be {(1 + int(steps), B, N, TARGET_DIM)}, got {trail_out.shape}")
+        if stats_out is not None and stats_out.nbytes < gs * B * GGS_STATS_DTYPE.itemsize:
+            raise ValueError(f"stats_out needs {gs * B} records")
+        ptrs, counts, shape, _keep = self._host_match_arrays(matches_dicts, B, N)
+        conf = ggs_config_struct(cfg)
+        with torch.cuda.device(self.device):
+            rc = self.lib.pdb_sample_loop_host_matches_ddim(self.handle, z.ctypes.data, draws.ctypes.data, B, N, int(steps), float(eta),
+                                                            gs, ptrs[0], ptrs[1], ptrs[2], counts, shape[0], shape[1], C.byref(conf),
+                                                            int(cond_start_step), pose_out.ctypes.data,
+                                                            trail_out.ctypes.data if trail_out is not None else None,
+                                                            stats_out.ctypes.data if stats_out is not None else None,
+                                                            _stream_ptr(self.device))
+        if rc == -1:
+            raise ValueError(self.lib.pdb_last_error(self.handle).decode())
+        self._ok(rc, "pdb_sample_loop_host_matches_ddim")
+        return pose_out
+
+    @staticmethod
+    def _host_match_arrays(matches_dicts, B: int, N: int):
+        """The pointer arrays of pdb_sample_loop_host_matches* for one matches_dict per sequence, and the arrays they point into."""
         if len(matches_dicts) != B:
             raise ValueError(f"{len(matches_dicts)} match sets for a batch of {B} sequences (one per sequence)")
         keep, shape = [], None
@@ -766,17 +840,7 @@ class Context:
             keep.append((kp1, kp2, i12))
         ptrs = [(C.c_void_p * B)(*[k[j].ctypes.data for k in keep]) for j in range(3)]
         counts = (C.c_int64 * B)(*[len(k[0]) for k in keep])
-        conf = ggs_config_struct(cfg)
-        with torch.cuda.device(self.device):
-            rc = self.lib.pdb_sample_loop_host_matches(self.handle, z.ctypes.data, draws.ctypes.data, B, N, ptrs[0], ptrs[1], ptrs[2],
-                                                       counts, shape[0], shape[1], C.byref(conf), int(cond_start_step),
-                                                       pose_out.ctypes.data, trail_out.ctypes.data if trail_out is not None else None,
-                                                       stats_out.ctypes.data if stats_out is not None else None,
-                                                       _stream_ptr(self.device))
-        if rc == -1:
-            raise ValueError(self.lib.pdb_last_error(self.handle).decode())
-        self._ok(rc, "pdb_sample_loop_host_matches")
-        return pose_out
+        return ptrs, counts, shape, keep
 
 
 def stats_to_numpy(stats: Optional[torch.Tensor]) -> Optional[np.ndarray]:

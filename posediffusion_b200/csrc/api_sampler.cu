@@ -1,4 +1,5 @@
-// C-ABI entry points: denoiser weights, denoiser forward, p_sample, p_sample_loop (device and host buffers).
+// C-ABI entry points: denoiser weights, denoiser forward, p_sample, p_sample_loop (device and host buffers), and its DDIM forms
+// (a strided prefix, and optionally guided DDIM jumps; DESIGN.md "Fewer-step sampling").
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -207,12 +208,13 @@ int enqueue_denoiser(Context* ctx, DenoiserRun run, cudaStream_t st, const Denoi
 
 // The sampling loop in two halves, so that a caller can do host work (match packing) between them while the first half runs:
 // loop_prefix enqueues x_T = draws[0] (gaussian_diffuser.py:289) and the unguided steps t = T-1 .. guide_below in ONE launch,
-// loop_guided the guided steps (denoiser -> posterior mean -> GGS in place).  A DDIM prefix (pdb_sample_loop_ddim) is k steps
-// on tables of virtual timesteps T-1 .. T-k; the guided steps that follow are the same DDPM steps either way.
+// loop_guided the guided steps (denoiser -> posterior mean -> GGS in place).  A DDIM prefix (pdb_sample_loop_ddim_guided) is k
+// steps on tables of virtual timesteps T-1 .. T-k; the guided steps that follow are today's DDPM steps, or g' < g DDIM jumps on
+// virtual timesteps g'-1 .. 0 of the same tables.
 struct LoopState {
   DenoiserRun run = {};
   int guide_below = 0;
-  int prefix_steps = 0;  // unguided steps before the guided ones: T - guide_below (DDPM) or k (DDIM); trail slot of guided step i = 1 + prefix_steps + i
+  int prefix_steps = 0;  // unguided steps before the guided ones: T - guide_below (DDPM) or k (DDIM); trail slot of guided step / jump i = 1 + prefix_steps + i
   bool first = true;
   size_t n = 0;
   float* pose = nullptr;
@@ -248,15 +250,18 @@ int loop_prefix(Context* ctx, const float* z_dev, const float* draws_dev, int ba
   return PDB_OK;
 }
 
+// jumps: NULL for the DDPM steps t = guide_below-1 .. 0, else the tables of make_ddim_tables, whose `jump_count` guided DDIM jumps
+// sit at virtual timesteps jump_count-1 .. 0 (below guide_below: the kernel leaves the mean, no noise, no trail slot).
 int loop_guided(Context* ctx, LoopState* loop, pdb_matches* const* problems, const pdb_ggs_config* cfg, pdb_ggs_stats* stats_dev,
-                cudaStream_t st) {
+                cudaStream_t st, const DenoiserDev* jumps = nullptr, int jump_count = 0) {
   DenoiserRun& run = loop->run;
-  for (int t = loop->guide_below - 1; t >= 0; --t) {
-    const int i = loop->guide_below - 1 - t;
+  const int steps = jumps ? jump_count : loop->guide_below;
+  for (int t = steps - 1; t >= 0; --t) {
+    const int i = steps - 1 - t;
     run.t_hi = run.t_lo = t;
     run.compute_zproj = loop->first ? 1 : 0;
     loop->first = false;
-    if (int rc = enqueue_denoiser(ctx, run, st)) return rc;
+    if (int rc = enqueue_denoiser(ctx, run, st, jumps)) return rc;
     pdb_ggs_stats* stats = stats_dev ? stats_dev + (size_t)i * run.batch : nullptr;
     if (int rc = enqueue_ggs(ctx, problems, run.batch, run.frames, loop->pose, cfg, stats, st)) return rc;
     if (loop->trail)
@@ -278,19 +283,21 @@ void schedule_f64(double beta_1, double beta_T, double* beta, double* abar) {
   }
 }
 
-// DDIM step table (Song et al. 2021, eq. 12; DESIGN.md "Fewer-step sampling").  Entries 0 .. k-1 (k = steps - guide_below) jump
-// tau_{k-i} -> tau_{k-i-1}, tau_j = (g - 1) + floor(j (T - g) / k), abar(-1) = 1; entries k .. steps-1 are the DDPM rows of the
-// guided timesteps g-1 .. 0.  False for k outside [1, T - g], eta < 0 or not finite, or an eta > 1 so large that
-// 1 - abar_s - sigma^2 < 0 at some jump.
-bool ddim_table(int steps, int guide_below, double eta, double beta_1, double beta_T, int32_t* t_out, float* coef_out) {
-  const int g = guide_below, k = steps - guide_below;
-  if (g < 0 || g > kT || k < 1 || k > kT - g || !std::isfinite(eta) || eta < 0.0) return false;
+// Guided jump times tau'_j = floor(j g / g') - 1, j = 0 .. g': tau'_{g'} = g - 1 (where the prefix lands), tau'_0 = -1 (x0).
+int guided_time(int j, int g, int gs) { return (int)((long long)j * g / gs) - 1; }
+
+// DDIM step table (Song et al. 2021, eq. 12; DESIGN.md "Fewer-step sampling").  Entries 0 .. k-1 (k = steps - guided_steps) jump
+// tau_{k-i} -> tau_{k-i-1}, tau_j = (g - 1) + floor(j (T - g) / k), abar(-1) = 1.  Entries k .. steps-1 are the guided tail: with
+// guided_steps == g the DDPM rows of timesteps g-1 .. 0, else g' DDIM jumps tau'_{g'-i} -> tau'_{g'-i-1} at the same eta.  False
+// for g' outside [min(1, g), g], k outside [1, T - g], eta < 0 or not finite, or an eta > 1 so large that 1 - abar_s - sigma^2 < 0
+// at some jump.
+bool ddim_table(int steps, int guide_below, int guided_steps, double eta, double beta_1, double beta_T, int32_t* t_out,
+                float* coef_out) {
+  const int g = guide_below, gs = guided_steps, k = steps - guided_steps;
+  if (g < 0 || g > kT || gs < (g > 0 ? 1 : 0) || gs > g || k < 1 || k > kT - g || !std::isfinite(eta) || eta < 0.0) return false;
   double beta[kT], abar[kT];
   schedule_f64(beta_1, beta_T, beta, abar);
-  for (int i = 0; i < k; ++i) {
-    const int j = k - i;
-    const int t = (g - 1) + (int)((long long)j * (kT - g) / k);
-    const int s = (g - 1) + (int)((long long)(j - 1) * (kT - g) / k);
+  auto jump = [&](int t, int s, int i) {
     const double at = abar[t], as = s < 0 ? 1.0 : abar[s];
     const double sigma = eta * std::sqrt((1.0 - as) / (1.0 - at)) * std::sqrt(1.0 - at / as);
     const double rest = 1.0 - as - sigma * sigma;
@@ -307,6 +314,16 @@ bool ddim_table(int steps, int guide_below, double eta, double beta_1, double be
     r[6] = (float)at;
     r[7] = (float)as;
     t_out[i] = t;
+    return true;
+  };
+  for (int i = 0; i < k; ++i) {
+    const int j = k - i;
+    if (!jump((g - 1) + (int)((long long)j * (kT - g) / k), (g - 1) + (int)((long long)(j - 1) * (kT - g) / k), i)) return false;
+  }
+  if (gs < g) {
+    for (int i = 0; i < gs; ++i)
+      if (!jump(guided_time(gs - i, g, gs), guided_time(gs - i - 1, g, gs), k + i)) return false;
+    return true;
   }
   float sched[kT * 8];
   pdb_schedule_table(sched, beta_1, beta_T);
@@ -317,35 +334,65 @@ bool ddim_table(int steps, int guide_below, double eta, double beta_1, double be
   return true;
 }
 
-// rows[kT - 1 - i] = src[t_i] (512 floats): the time-embedding block of step i's timestep at its virtual timestep
-struct RowMap { int src[kT]; };
+// dst[v_i] = src[t_i] (512 floats): the time-embedding block of step i's real timestep at its virtual timestep
+struct RowMap { int dst[kT]; int src[kT]; };
 __global__ void gather_tproj_kernel(const float* __restrict__ src, float* __restrict__ dst, RowMap map) {
   const int i = blockIdx.x;
-  for (int c = threadIdx.x; c < kDM; c += blockDim.x) dst[(size_t)(kT - 1 - i) * kDM + c] = src[(size_t)map.src[i] * kDM + c];
+  for (int c = threadIdx.x; c < kDM; c += blockDim.x) dst[(size_t)map.dst[i] * kDM + c] = src[(size_t)map.src[i] * kDM + c];
 }
 
-// The k-step DDIM prefix as the kernels see it: a copy of the weight descriptor whose per-timestep tables are indexed by the virtual
-// timestep v = T-1-i of prefix step i -- sched[v] = its DDIM coefficient row, tproj[v] = the time-embedding block of its real
-// timestep.  The DDPM loop over v = T-1 .. T-k then IS the DDIM prefix, draw and trail slot 1 + i included.  The tables live in a
-// context-owned buffer at a fixed address, rewritten (stream-ordered) before each loop.
-int make_ddim_tables(Context* ctx, const int32_t* tab_t, const float* tab_coef, int k, cudaStream_t st, DenoiserDev* out) {
+// A DDIM loop as the kernels see it: a copy of the weight descriptor whose per-timestep tables are indexed by virtual timesteps --
+// sched[v] = a step's DDIM coefficient row, tproj[v] = the time-embedding block of its real timestep.  Prefix step i sits at
+// v = T-1-i, so the DDPM loop over v = T-1 .. T-k IS the DDIM prefix, draw and trail slot 1 + i included.  The `jumps` guided
+// jumps (table entries k ..; 0 when the tail stays DDPM) sit at v = jumps-1 .. 0: below guide_below, so the kernel adds no noise
+// and writes no trail slot for them; jumps <= g <= T - k keeps the two ranges apart.  The tables live in a context-owned buffer at
+// a fixed address, rewritten (stream-ordered) before each loop.
+int make_ddim_tables(Context* ctx, const int32_t* tab_t, const float* tab_coef, int k, int jumps, cudaStream_t st, DenoiserDev* out) {
   const size_t sched_floats = (size_t)kT * 8, bytes = sizeof(float) * (sched_floats + (size_t)kT * kDM);
   if (!ctx->step_tab) PDB_CUDA(ctx, cudaMalloc(&ctx->step_tab, bytes));
   float* vsched = static_cast<float*>(ctx->step_tab);
   float* vtproj = vsched + sched_floats;
   float rows[kT * 8] = {};
   RowMap map = {};
-  for (int i = 0; i < k; ++i) {
-    std::memcpy(rows + (size_t)(kT - 1 - i) * 8, tab_coef + (size_t)i * 8, sizeof(float) * 8);
+  for (int i = 0; i < k + jumps; ++i) {
+    const int v = i < k ? kT - 1 - i : k + jumps - 1 - i;
+    std::memcpy(rows + (size_t)v * 8, tab_coef + (size_t)i * 8, sizeof(float) * 8);
+    map.dst[i] = v;
     map.src[i] = tab_t[i];
   }
   PDB_CUDA(ctx, cudaMemcpyAsync(vsched, rows, sizeof(rows), cudaMemcpyHostToDevice, st));
   *out = ctx->weights->dev;
-  gather_tproj_kernel<<<k, 128, 0, st>>>(out->tproj, vtproj, map);
+  gather_tproj_kernel<<<k + jumps, 128, 0, st>>>(out->tproj, vtproj, map);
   PDB_CUDA(ctx, cudaGetLastError());
   ctx->launches += 1;
   out->tproj = vtproj;
   out->sched = vsched;
+  return PDB_OK;
+}
+
+int clamp_guided(int cond_start_step) { return cond_start_step < 0 ? 0 : (cond_start_step > kT ? kT : cond_start_step); }
+
+// A DDIM loop's step table, computed and checked before anything is enqueued.
+struct DdimPlan {
+  int g = 0;      // guided timesteps: clamp(cond_start_step, 0, T)
+  int k = 0;      // unguided prefix steps
+  int jumps = 0;  // guided DDIM jumps on the step tables; 0 when the tail is the g DDPM steps on the weights' own tables
+  int guided = 0; // denoiser evaluations of the guided tail (g' = jumps, or g)
+  int32_t t[kT];
+  float coef[kT * 8];
+};
+
+int ddim_plan(Context* ctx, int steps, double eta, int guided_steps, int cond_start_step, DdimPlan* p) {
+  const int g = clamp_guided(cond_start_step);
+  if (!ddim_table(steps, g, guided_steps, eta, 1e-4, 0.1, p->t, p->coef))
+    return ctx->fail(PDB_ERR_INVALID,
+                     "DDIM: %d denoiser steps, %d of them over %d guided timesteps (the guided tail needs %d .. %d, the unguided prefix "
+                     "1 .. %d) and eta %g (>= 0, finite)",
+                     steps, guided_steps, g, g > 0 ? 1 : 0, g, kT - g, eta);
+  p->g = g;
+  p->k = steps - guided_steps;
+  p->guided = guided_steps;
+  p->jumps = guided_steps < g ? guided_steps : 0;
   return PDB_OK;
 }
 
@@ -641,13 +688,26 @@ int pdb_sample_loop(pdb_context* c, const float* z_dev, const float* draws_dev, 
 }
 
 int pdb_ddim_table(int32_t steps, int32_t guide_below, double eta, double beta_1, double beta_T, int32_t* t_out, float* coef_out) {
+  return pdb_ddim_table_guided(steps, guide_below, guide_below, eta, beta_1, beta_T, t_out, coef_out);
+}
+
+int pdb_ddim_table_guided(int32_t steps, int32_t guide_below, int32_t guided_steps, double eta, double beta_1, double beta_T,
+                          int32_t* t_out, float* coef_out) {
   if (!t_out || !coef_out) return PDB_ERR_INVALID;
-  return ddim_table(steps, guide_below, eta, beta_1, beta_T, t_out, coef_out) ? PDB_OK : PDB_ERR_INVALID;
+  return ddim_table(steps, guide_below, guided_steps, eta, beta_1, beta_T, t_out, coef_out) ? PDB_OK : PDB_ERR_INVALID;
 }
 
 int pdb_sample_loop_ddim(pdb_context* c, const float* z_dev, const float* draws_dev, int32_t batch, int32_t frames, int32_t steps,
                          double eta, pdb_matches* const* problems, int32_t n_problems, const pdb_ggs_config* cfg, int32_t cond_start_step,
                          float* pose_dev, float* trail_dev, pdb_ggs_stats* stats_dev, void* stream) {
+  return pdb_sample_loop_ddim_guided(c, z_dev, draws_dev, batch, frames, steps, eta, clamp_guided(cond_start_step), problems,
+                                     n_problems, cfg, cond_start_step, pose_dev, trail_dev, stats_dev, stream);
+}
+
+int pdb_sample_loop_ddim_guided(pdb_context* c, const float* z_dev, const float* draws_dev, int32_t batch, int32_t frames,
+                                int32_t steps, double eta, int32_t guided_steps, pdb_matches* const* problems, int32_t n_problems,
+                                const pdb_ggs_config* cfg, int32_t cond_start_step, float* pose_dev, float* trail_dev,
+                                pdb_ggs_stats* stats_dev, void* stream) {
   if (!c) return PDB_ERR_INVALID;
   Context* ctx = reinterpret_cast<Context*>(c);
   if (!z_dev || !draws_dev || !pose_dev) return ctx->fail(PDB_ERR_INVALID, "null argument");
@@ -656,25 +716,21 @@ int pdb_sample_loop_ddim(pdb_context* c, const float* z_dev, const float* draws_
   if (problems && !cfg) return ctx->fail(PDB_ERR_INVALID, "GGS config missing");
   if (problems && n_problems != batch)
     return ctx->fail(PDB_ERR_INVALID, "%d match sets for a batch of %d sequences (one per sequence)", n_problems, batch);
-  const int g = cond_start_step < 0 ? 0 : (cond_start_step > kT ? kT : cond_start_step);
-  int32_t tab_t[kT];
-  float tab_coef[kT * 8];
-  if (!ddim_table(steps, g, eta, 1e-4, 0.1, tab_t, tab_coef))
-    return ctx->fail(PDB_ERR_INVALID, "DDIM: %d denoiser steps with %d guided (the unguided prefix needs 1 .. %d) and eta %g (>= 0, finite)",
-                     steps, g, kT - g, eta);
+  DdimPlan plan;
+  if (int rc = ddim_plan(ctx, steps, eta, guided_steps, cond_start_step, &plan)) return rc;
   if (problems)
     if (int rc = check_ggs_problems(ctx, problems, batch, frames)) return rc;
   if (!ctx->weights) return ctx->fail(PDB_ERR_STATE, "denoiser weights not loaded (pdb_denoiser_load)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   PDB_CUDA(ctx, cudaSetDevice(ctx->device));
   DenoiserDev tables;
-  if (int rc = make_ddim_tables(ctx, tab_t, tab_coef, steps - g, st, &tables)) return rc;
+  if (int rc = make_ddim_tables(ctx, plan.t, plan.coef, plan.k, plan.jumps, st, &tables)) return rc;
   LoopState loop;
-  if (int rc = loop_prefix(ctx, z_dev, draws_dev, batch, frames, g, pose_dev, trail_dev, st, &loop, &tables, steps - g,
+  if (int rc = loop_prefix(ctx, z_dev, draws_dev, batch, frames, plan.g, pose_dev, trail_dev, st, &loop, &tables, plan.k,
                            eta > 0.0 ? draws_dev : nullptr))
     return rc;
   if (!problems) return PDB_OK;  // cond_start_step > 0 without match sets: the prefix alone, x_{g-1} (generic cond_fn callers)
-  return loop_guided(ctx, &loop, problems, cfg, stats_dev, st);
+  return loop_guided(ctx, &loop, problems, cfg, stats_dev, st, plan.jumps ? &tables : nullptr, plan.jumps);
 }
 
 int pdb_sample_loop_host(pdb_context* c, const float* z_host, const float* draws_host, int32_t batch, int32_t frames,
@@ -714,23 +770,21 @@ int pdb_sample_loop_host(pdb_context* c, const float* z_host, const float* draws
 
 // The end-to-end call of a guided run that starts from the reference's match format (host arrays, one match set per sequence):
 // the match sets are packed and uploaded WHILE the unguided prefix of the loop (t = T-1 .. cond_start_step, one launch) runs on
-// the GPU -- the packer is host work plus a copy on its own stream, the prefix does not need the matches.
-int pdb_sample_loop_host_matches(pdb_context* c, const float* z_host, const float* draws_host, int32_t batch, int32_t frames,
-                                 const double* const* kp1, const double* const* kp2, const int64_t* const* i12,
-                                 const int64_t* m_total, int32_t height, int32_t width, const pdb_ggs_config* cfg,
-                                 int32_t cond_start_step, float* pose_host, float* trail_host, pdb_ggs_stats* stats_host,
-                                 void* stream) {
-  if (!c) return PDB_ERR_INVALID;
+// the GPU -- the packer is host work plus a copy on its own stream, the prefix does not need the matches.  `ddim` NULL: the DDPM
+// loop; else the checked plan of a DDIM loop (pdb_sample_loop_host_matches_ddim).
+static int host_matches_loop(pdb_context* c, const float* z_host, const float* draws_host, int32_t batch, int32_t frames,
+                             const double* const* kp1, const double* const* kp2, const int64_t* const* i12, const int64_t* m_total,
+                             int32_t height, int32_t width, const pdb_ggs_config* cfg, int32_t cond_start_step, float* pose_host,
+                             float* trail_host, pdb_ggs_stats* stats_host, void* stream, const DdimPlan* ddim, double eta) {
   Context* ctx = reinterpret_cast<Context*>(c);
-  if (!z_host || !draws_host || !pose_host || !kp1 || !kp2 || !i12 || !m_total || !cfg)
-    return ctx->fail(PDB_ERR_INVALID, "null argument");
-  if (batch < 1 || frames < 1) return ctx->fail(PDB_ERR_INVALID, "bad batch / frames");
+  if (ddim && !ctx->weights) return ctx->fail(PDB_ERR_STATE, "denoiser weights not loaded (pdb_denoiser_load)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   PDB_CUDA(ctx, cudaSetDevice(ctx->device));
   if (!ctx->pack_stream) PDB_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->pack_stream, cudaStreamNonBlocking));
   const size_t S = (size_t)batch * frames, n = S * kTargetDim;
-  const int guided = cond_start_step < 0 ? 0 : (cond_start_step > kT ? kT : cond_start_step);
-  const size_t f_z = S * kZ, f_draws = (size_t)(kT + 1) * n, f_pose = n, f_trail = trail_host ? (size_t)(kT + 1) * n : 0;
+  const int guided = ddim ? ddim->guided : clamp_guided(cond_start_step);
+  const size_t draw_slots = ddim ? (eta > 0.0 ? 1 + ddim->k : 1) : kT + 1, trail_slots = ddim ? 1 + ddim->k + ddim->guided : kT + 1;
+  const size_t f_z = S * kZ, f_draws = draw_slots * n, f_pose = n, f_trail = trail_host ? trail_slots * n : 0;
   const size_t stats_bytes = stats_host ? sizeof(pdb_ggs_stats) * (size_t)guided * batch : 0;
   const size_t bytes = sizeof(float) * (f_z + f_draws + f_pose + f_trail) + stats_bytes + 256;
   if (int rc = ensure_buffer(ctx, &ctx->stage, &ctx->stage_bytes, bytes)) return rc;
@@ -743,14 +797,23 @@ int pdb_sample_loop_host_matches(pdb_context* c, const float* z_host, const floa
   PDB_CUDA(ctx, cudaMemcpyAsync(draws_dev, draws_host, sizeof(float) * f_draws, cudaMemcpyHostToDevice, st));
   if (stats_dev) PDB_CUDA(ctx, cudaMemsetAsync(stats_dev, 0, stats_bytes, st));
   LoopState loop;
-  if (int rc = loop_prefix(ctx, z_dev, draws_dev, batch, frames, guided, pose_dev, trail_dev, st, &loop)) return rc;
+  DenoiserDev tables;
+  if (ddim) {
+    if (int rc = make_ddim_tables(ctx, ddim->t, ddim->coef, ddim->k, ddim->jumps, st, &tables)) return rc;
+    if (int rc = loop_prefix(ctx, z_dev, draws_dev, batch, frames, ddim->g, pose_dev, trail_dev, st, &loop, &tables, ddim->k,
+                             eta > 0.0 ? draws_dev : nullptr))
+      return rc;
+  } else if (int rc = loop_prefix(ctx, z_dev, draws_dev, batch, frames, guided, pose_dev, trail_dev, st, &loop)) {
+    return rc;
+  }
   // ---- host: pack while the prefix runs (pdb_matches_pack returns once ITS stream has taken the upload) ----
   std::vector<pdb_matches*> sets((size_t)batch, nullptr);
   int rc = PDB_OK;
   for (int b = 0; b < batch && rc == PDB_OK; ++b)
     rc = pdb_matches_pack(c, kp1[b], kp2[b], i12[b], m_total[b], frames, height, width, 0, ctx->pack_stream, &sets[b]);
   if (rc == PDB_OK) rc = check_ggs_problems(ctx, sets.data(), batch, frames);
-  if (rc == PDB_OK) rc = loop_guided(ctx, &loop, sets.data(), cfg, stats_dev, st);
+  const bool jumps = ddim && ddim->jumps;
+  if (rc == PDB_OK) rc = loop_guided(ctx, &loop, sets.data(), cfg, stats_dev, st, jumps ? &tables : nullptr, jumps ? ddim->jumps : 0);
   cudaError_t err = cudaSuccess;
   if (rc == PDB_OK) {
     err = cudaMemcpyAsync(pose_host, pose_dev, sizeof(float) * f_pose, cudaMemcpyDeviceToHost, st);
@@ -764,6 +827,42 @@ int pdb_sample_loop_host_matches(pdb_context* c, const float* z_host, const floa
   if (err != cudaSuccess || sync != cudaSuccess)
     return ctx->fail(PDB_ERR_CUDA, "sample loop failed: %s", cudaGetErrorString(err != cudaSuccess ? err : sync));
   return PDB_OK;
+}
+
+static int host_matches_check(pdb_context* c, const float* z_host, const float* draws_host, int32_t batch, int32_t frames,
+                              const double* const* kp1, const double* const* kp2, const int64_t* const* i12, const int64_t* m_total,
+                              const pdb_ggs_config* cfg, const float* pose_host) {
+  Context* ctx = reinterpret_cast<Context*>(c);
+  if (!z_host || !draws_host || !pose_host || !kp1 || !kp2 || !i12 || !m_total || !cfg)
+    return ctx->fail(PDB_ERR_INVALID, "null argument");
+  if (batch < 1 || frames < 1) return ctx->fail(PDB_ERR_INVALID, "bad batch / frames");
+  return PDB_OK;
+}
+
+int pdb_sample_loop_host_matches(pdb_context* c, const float* z_host, const float* draws_host, int32_t batch, int32_t frames,
+                                 const double* const* kp1, const double* const* kp2, const int64_t* const* i12,
+                                 const int64_t* m_total, int32_t height, int32_t width, const pdb_ggs_config* cfg,
+                                 int32_t cond_start_step, float* pose_host, float* trail_host, pdb_ggs_stats* stats_host,
+                                 void* stream) {
+  if (!c) return PDB_ERR_INVALID;
+  if (int rc = host_matches_check(c, z_host, draws_host, batch, frames, kp1, kp2, i12, m_total, cfg, pose_host)) return rc;
+  return host_matches_loop(c, z_host, draws_host, batch, frames, kp1, kp2, i12, m_total, height, width, cfg, cond_start_step,
+                           pose_host, trail_host, stats_host, stream, nullptr, 0.0);
+}
+
+int pdb_sample_loop_host_matches_ddim(pdb_context* c, const float* z_host, const float* draws_host, int32_t batch, int32_t frames,
+                                      int32_t steps, double eta, int32_t guided_steps, const double* const* kp1,
+                                      const double* const* kp2, const int64_t* const* i12, const int64_t* m_total, int32_t height,
+                                      int32_t width, const pdb_ggs_config* cfg, int32_t cond_start_step, float* pose_host,
+                                      float* trail_host, pdb_ggs_stats* stats_host, void* stream) {
+  if (!c) return PDB_ERR_INVALID;
+  Context* ctx = reinterpret_cast<Context*>(c);
+  if (int rc = host_matches_check(c, z_host, draws_host, batch, frames, kp1, kp2, i12, m_total, cfg, pose_host)) return rc;
+  if (frames > PDB_MAX_FRAMES) return ctx->fail(PDB_ERR_LIMIT, "frames %d > PDB_MAX_FRAMES", frames);
+  DdimPlan plan;
+  if (int rc = ddim_plan(ctx, steps, eta, guided_steps, cond_start_step, &plan)) return rc;
+  return host_matches_loop(c, z_host, draws_host, batch, frames, kp1, kp2, i12, m_total, height, width, cfg, cond_start_step,
+                           pose_host, trail_host, stats_host, stream, &plan, eta);
 }
 
 }  // extern "C"

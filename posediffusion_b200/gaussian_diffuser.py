@@ -10,8 +10,9 @@ still CUDA-only.  Gaussian draws come from torch's generator on the sampler's de
 order (one `randn(shape)` then one `randn_like` per unguided step with t > 0, :289, :278).
 
 `ddim_sample` is the fewer-step sampling the reference's `sampling_timesteps` argument names but never built (:79, :150-154,
-:303-306): the unguided prefix in k < 100 DDIM steps (Song et al. 2021, eq. 12), then exactly `p_sample_loop`'s guided tail.
-`sample` / `p_sample_loop` do not change: DDIM is opt-in.
+:303-306): the unguided prefix in k < 100 DDIM steps (Song et al. 2021, eq. 12), then exactly `p_sample_loop`'s guided tail, or,
+with `guided_steps`, that tail in fewer DDIM jumps each followed by the guidance.  `sample` / `p_sample_loop` do not change: DDIM
+is opt-in.
 """
 from __future__ import annotations
 
@@ -165,18 +166,24 @@ class GaussianDiffusion(nn.Module):
 
     @torch.no_grad()
     def ddim_sample(self, shape, z: torch.Tensor, cond_fn: Optional[Callable] = None, cond_start_step: int = 0,
-                    sampling_timesteps: Optional[int] = None, eta: float = 0.0, draws: Optional[torch.Tensor] = None):
-        """(pose [B,N,9], trail [1 + k + g, B, N, 9]) in `sampling_timesteps` denoiser evaluations (default: the constructor's
-        `sampling_timesteps`).  g = clamp(cond_start_step, 0, 100) guided steps when cond_fn is given (else 0) run exactly as in
-        `p_sample_loop`; the k = sampling_timesteps - g unguided ones are DDIM jumps with noise scale eta (0: deterministic, 1: the
-        DDPM posterior variance; at k = 100 - g and eta = 1 the steps are DDPM's).  k and eta trade speed against sample quality;
-        the released checkpoint's pose accuracy under DDIM has not been measured.  ValueError for k outside [1, 100 - g] or an eta
-        that is negative or not finite.  `draws` as `ddim_draws` makes them."""
+                    sampling_timesteps: Optional[int] = None, eta: float = 0.0, draws: Optional[torch.Tensor] = None,
+                    guided_steps: Optional[int] = None):
+        """(pose [B,N,9], trail [1 + k + g', B, N, 9]) in `sampling_timesteps` denoiser evaluations (default: the constructor's
+        `sampling_timesteps`).  The guided tail covers g = clamp(cond_start_step, 0, 100) timesteps when cond_fn is given (else 0).
+        With `guided_steps` None or g it runs exactly as in `p_sample_loop`: g DDPM steps, each followed by cond_fn.  With
+        g' = guided_steps < g it takes g' DDIM jumps over timesteps g-1 .. -1 (jump times floor(j g / g') - 1), each to the DDIM mean
+        without noise and followed by cond_fn on that mean; cond_fn's own settings (the GGS iteration counts of GGS_cfg) are not
+        rescaled by the stride.  The k = sampling_timesteps - g' unguided steps are DDIM jumps with noise scale eta (0:
+        deterministic, 1: the DDPM posterior variance; at k = 100 - g and eta = 1 the steps are DDPM's).  k, g' and eta trade speed
+        against sample quality; the released checkpoint's pose accuracy under DDIM has not been measured.  ValueError for k outside
+        [1, 100 - g], g' outside [1, g] or given without guidance, or an eta that is negative or not finite.  `draws` as
+        `ddim_draws` makes them."""
         self._require_native()
         steps = self.sampling_timesteps if sampling_timesteps is None else int(sampling_timesteps)
         guided = max(0, min(int(cond_start_step), self.num_timesteps)) if cond_fn is not None else 0
         eta = float(eta)
-        k = _native.ddim_check(steps, guided, eta)
+        k = _native.ddim_check(steps, guided, eta, guided_steps)
+        gs = guided if guided_steps is None else int(guided_steps)
         device = self.betas.device
         ctx = self.model.native_context()
         z = z.contiguous().float()
@@ -188,18 +195,29 @@ class GaussianDiffusion(nn.Module):
             if cond_fn is not None:
                 cfg = cond_fn.keywords["GGS_cfg"]
                 problems = packed_matches(ctx, cond_fn.keywords["matches_dict"])
-            pose, trail, stats = ctx.sample_loop_ddim(z, draws, steps, eta, problems, cfg, guided)
+            pose, trail, stats = ctx.sample_loop_ddim(z, draws, steps, eta, problems, cfg, guided, guided_steps=guided_steps)
             self.last_ggs_stats = stats
             if stats is not None and bool(cfg.get("verbose", True)):
+                starts = _native.guided_times(guided, gs)[:0:-1] if gs else []  # the real timestep each guided step starts from
                 rows = _native.stats_to_numpy(stats).reshape(-1, shape[0])
                 for i, per_step in enumerate(rows):
                     for row in per_step:
-                        print("\n".join(format_log(guided - 1 - i, row)))
+                        print("\n".join(format_log(starts[i], row)))
             return pose, trail
-        # generic cond_fn: the DDIM prefix natively (it stops at x_{g-1}), then the guided DDPM steps around the native step
-        pose, trail, _ = ctx.sample_loop_ddim(z, draws, steps, eta, None, None, guided)
-        for i, t in enumerate(reversed(range(guided))):
-            _, mean, _ = ctx.p_sample(pose, t, z, None)
+        # generic cond_fn: the DDIM prefix natively (it stops at x_{g-1}), then the guided steps around the native step
+        pose, trail, _ = ctx.sample_loop_ddim(z, draws, steps, eta, None, None, guided, guided_steps=guided_steps)
+        if gs == guided:  # DDPM steps
+            for i, t in enumerate(reversed(range(guided))):
+                _, mean, _ = ctx.p_sample(pose, t, z, None)
+                pose = cond_fn(mean, t)
+                trail[1 + k + i] = pose
+            return pose, trail
+        t_tab, coef = _native.ddim_table(steps, guided, eta, guided_steps=gs)
+        for i in range(gs):  # DDIM jumps: the table row applied to the native network output, no noise
+            t = int(t_tab[k + i])
+            a, b, c1, c2 = (float(v) for v in coef[k + i, :4])
+            eps = ctx.denoiser_forward(pose, t, z)
+            mean = c1 * (a * pose - b * eps) + c2 * pose
             pose = cond_fn(mean, t)
             trail[1 + k + i] = pose
         return pose, trail

@@ -59,7 +59,9 @@ class PoseDiffusionModel(nn.Module):
 
     def forward(self, image: Optional[torch.Tensor] = None, gt_cameras=None, sequence_name: Optional[List[str]] = None,
                 cond_fn=None, cond_start_step=0, training=True, batch_repeat=-1, z: Optional[torch.Tensor] = None,
-                sampling_timesteps: Optional[int] = None, eta: float = 0.0):
+                sampling_timesteps: Optional[int] = None, eta: float = 0.0, guided_steps: Optional[int] = None):
+        if guided_steps is not None and sampling_timesteps is None:
+            raise ValueError("guided_steps is a DDIM option: pass sampling_timesteps too")
         if z is None:
             if self.image_feature_extractor is None or image is None:
                 raise ValueError("no image feature extractor configured: pass precomputed features as z=[B,N,384]")
@@ -92,10 +94,10 @@ class PoseDiffusionModel(nn.Module):
             pose_encoding, _trajectory = self.diffuser.sample(
                 shape=[B, N, self.target_dim], z=z, cond_fn=cond_fn, cond_start_step=cond_start_step
             )
-        else:  # fewer denoiser steps: DDIM over the unguided prefix (GaussianDiffusion.ddim_sample)
+        else:  # fewer denoiser steps: DDIM over the unguided prefix, and over the guided tail with guided_steps (ddim_sample)
             pose_encoding, _trajectory = self.diffuser.ddim_sample(
                 shape=[B, N, self.target_dim], z=z, cond_fn=cond_fn, cond_start_step=cond_start_step,
-                sampling_timesteps=sampling_timesteps, eta=eta
+                sampling_timesteps=sampling_timesteps, eta=eta, guided_steps=guided_steps
             )
         pred_cameras = pose_encoding_to_camera(pose_encoding, pose_encoding_type=self.pose_encoding_type)
         return {"pred_cameras": pred_cameras, "z": z}
