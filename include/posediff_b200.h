@@ -222,7 +222,11 @@ int pdb_ggs(pdb_context* ctx, pdb_matches* const* problems, int32_t batch, float
  * problems == NULL -> no guidance; otherwise problems[n_problems] holds ONE match set per sequence: n_problems must equal
  * `batch` and every set must have been packed for `frames` frames (PDB_ERR_INVALID otherwise -- the kernels index
  * problems[b] and stride the pose by the set's frame count).  cond_start_step as in p_sample (:270).  trail_dev may be NULL, else
- * [T+1, B, N, 9].  stats_dev may be NULL, else [cond_start_step, batch] records (row 0 = first guided step). */
+ * [T+1, B, N, 9].  stats_dev may be NULL, else [cond_start_step, batch] records (row 0 = first guided step).
+ * Every sampling-loop entry point refuses its arguments before anything is enqueued: NULL pointers, batch or frames < 1,
+ * frames > PDB_MAX_FRAMES (PDB_ERR_LIMIT), no weights loaded (PDB_ERR_STATE), match sets without cfg or as above, cfg->iter_num
+ * < 0, and the DDIM entries' step-table refusals.  Only a match set that fails to pack in pdb_sample_loop_host_matches* is
+ * found later, while the unguided steps run. */
 int pdb_sample_loop(pdb_context* ctx, const float* z_dev, const float* draws_dev, int32_t batch, int32_t frames,
                     pdb_matches* const* problems, int32_t n_problems, const pdb_ggs_config* cfg,
                     int32_t cond_start_step, float* pose_dev, float* trail_dev, pdb_ggs_stats* stats_dev, void* stream);
@@ -260,7 +264,8 @@ int pdb_sample_loop_host(pdb_context* ctx, const float* z_host, const float* dra
  * (int64 [m_total[b], 2]) are the HOST arrays of sequence b's matches_dict (util/match_extraction.py:50-77), as pdb_matches_pack
  * takes them.  The sets are packed and uploaded while the unguided steps t = T-1 .. cond_start_step already run on the GPU, then
  * the guided steps follow; the packed sets are released before the call returns.  Results are those of pdb_matches_pack +
- * pdb_sample_loop_host.  cfg must not be NULL. */
+ * pdb_sample_loop_host.  cfg must not be NULL.  A set that fails to pack (e.g. an i12 index outside the frames) is refused
+ * while the unguided steps run: the stream is then synchronised and the sets packed so far are released. */
 int pdb_sample_loop_host_matches(pdb_context* ctx, const float* z_host, const float* draws_host, int32_t batch, int32_t frames,
                                  const double* const* kp1, const double* const* kp2, const int64_t* const* i12,
                                  const int64_t* m_total, int32_t height, int32_t width, const pdb_ggs_config* cfg,
@@ -269,7 +274,8 @@ int pdb_sample_loop_host_matches(pdb_context* ctx, const float* z_host, const fl
 
 /* pdb_sample_loop_host_matches on the loop of pdb_sample_loop_ddim_guided: the sets are packed while the DDIM prefix runs.
  * draws_host [1 + k, B, N, 9] for eta > 0, [1, B, N, 9] for eta == 0; trail_host [1 + k + g', B, N, 9]; stats_host [g', batch].
- * The same refusals as pdb_sample_loop_ddim_guided, before anything is enqueued. */
+ * The same refusals as pdb_sample_loop_ddim_guided, before anything is enqueued; a set that fails to pack as in
+ * pdb_sample_loop_host_matches. */
 int pdb_sample_loop_host_matches_ddim(pdb_context* ctx, const float* z_host, const float* draws_host, int32_t batch, int32_t frames,
                                       int32_t steps, double eta, int32_t guided_steps, const double* const* kp1,
                                       const double* const* kp2, const int64_t* const* i12, const int64_t* m_total, int32_t height,

@@ -209,6 +209,11 @@ def guided_times(g: int, guided_steps: int) -> List[int]:
     return [(j * int(g)) // int(guided_steps) - 1 for j in range(int(guided_steps) + 1)]
 
 
+def clamp_guided(cond_start_step: int) -> int:
+    """g = clamp(cond_start_step, 0, 100): the timesteps a sampling loop guides."""
+    return max(0, min(int(cond_start_step), NUM_TIMESTEPS))
+
+
 def ddim_check(steps: int, guided: int, eta: float, guided_steps: Optional[int] = None) -> int:
     """k = steps - g' unguided DDIM steps (g' = `guided_steps`, default `guided`), or ValueError (the library's own check, mirrored
     so that nothing is enqueued)."""
@@ -704,27 +709,33 @@ class Context:
                                   stats.data_ptr() if want_stats else None, _stream_ptr(self.device)), "pdb_ggs")
         return stats
 
-    def sample_loop(self, z: torch.Tensor, draws: torch.Tensor, problems: Optional[Sequence[Matches]], cfg: Optional[Dict],
-                    cond_start_step: int, want_trail: bool = True, want_stats: bool = True):
+    def _device_loop(self, entry: str, ddim_args, z: torch.Tensor, draws: torch.Tensor, draw_slots: int, trail_slots: int,
+                     stats_rows: int, problems, cfg, cond_start_step: int, want_trail: bool, want_stats: bool):
+        """Check the shapes, allocate pose [B, N, 9], trail [trail_slots, B, N, 9] and stats [stats_rows, B] and run the device
+        entry `entry` (`ddim_args` go between the frame count and the match sets)."""
         B, N, _ = z.shape
         _check_dev(z, "z", self.device, (B, N, Z_DIM))
-        _check_dev(draws, "draws", self.device, (NUM_TIMESTEPS + 1, B, N, TARGET_DIM))
-        pose = torch.empty(B, N, TARGET_DIM, device=self.device)
-        trail = torch.empty(NUM_TIMESTEPS + 1, B, N, TARGET_DIM, device=self.device) if want_trail else None
-        guided = max(0, min(int(cond_start_step), NUM_TIMESTEPS)) if problems else 0
+        _check_dev(draws, "draws", self.device, (draw_slots, B, N, TARGET_DIM))
         if problems:
             self._check_problems(problems, B, N)
+        pose = torch.empty(B, N, TARGET_DIM, device=self.device)
+        trail = torch.empty(trail_slots, B, N, TARGET_DIM, device=self.device) if want_trail else None
         stats = None
-        if want_stats and guided:
-            stats = torch.zeros(guided * B * GGS_STATS_DTYPE.itemsize, dtype=torch.uint8, device=self.device)
+        if want_stats and problems and stats_rows:
+            stats = torch.zeros(stats_rows * B * GGS_STATS_DTYPE.itemsize, dtype=torch.uint8, device=self.device)
         conf = ggs_config_struct(cfg) if problems else None
-        self._ok(self.lib.pdb_sample_loop(self.handle, z.data_ptr(), draws.data_ptr(), B, N,
+        self._ok(getattr(self.lib, entry)(self.handle, z.data_ptr(), draws.data_ptr(), B, N, *ddim_args,
                                           self._problem_array(problems) if problems else None, len(problems) if problems else 0,
                                           C.byref(conf) if conf is not None else None, int(cond_start_step), pose.data_ptr(),
-                                          trail.data_ptr() if want_trail else None,
-                                          stats.data_ptr() if stats is not None else None, _stream_ptr(self.device)),
-                 "pdb_sample_loop")
+                                          trail.data_ptr() if want_trail else None, stats.data_ptr() if stats is not None else None,
+                                          _stream_ptr(self.device)), entry)
         return pose, trail, stats
+
+    def sample_loop(self, z: torch.Tensor, draws: torch.Tensor, problems: Optional[Sequence[Matches]], cfg: Optional[Dict],
+                    cond_start_step: int, want_trail: bool = True, want_stats: bool = True):
+        guided = clamp_guided(cond_start_step) if problems else 0
+        return self._device_loop("pdb_sample_loop", (), z, draws, NUM_TIMESTEPS + 1, NUM_TIMESTEPS + 1, guided, problems, cfg,
+                                 cond_start_step, want_trail, want_stats)
 
     def sample_loop_ddim(self, z: torch.Tensor, draws: torch.Tensor, steps: int, eta: float, problems: Optional[Sequence[Matches]],
                          cfg: Optional[Dict], cond_start_step: int, want_trail: bool = True, want_stats: bool = True,
@@ -733,32 +744,30 @@ class Context:
         g = clamp(cond_start_step) timesteps takes g' = `guided_steps` (default g) jumps, the prefix k = steps - g'.  draws
         [1 + k, B, N, 9] for eta > 0, [1, B, N, 9] for eta == 0.  Without problems and with cond_start_step > 0 only the prefix runs
         (pose = x_{g-1})."""
-        B, N, _ = z.shape
-        _check_dev(z, "z", self.device, (B, N, Z_DIM))
-        guided = max(0, min(int(cond_start_step), NUM_TIMESTEPS))
+        guided = clamp_guided(cond_start_step)
         k = ddim_check(steps, guided, eta, guided_steps)
         gs = guided if guided_steps is None else int(guided_steps)
-        _check_dev(draws, "draws", self.device, (1 + k if eta > 0 else 1, B, N, TARGET_DIM))
-        if problems:
-            self._check_problems(problems, B, N)
-        pose = torch.empty(B, N, TARGET_DIM, device=self.device)
-        trail = torch.empty(1 + int(steps), B, N, TARGET_DIM, device=self.device) if want_trail else None
-        stats = None
-        if want_stats and problems and gs:
-            stats = torch.zeros(gs * B * GGS_STATS_DTYPE.itemsize, dtype=torch.uint8, device=self.device)
-        conf = ggs_config_struct(cfg) if problems else None
-        self._ok(self.lib.pdb_sample_loop_ddim_guided(self.handle, z.data_ptr(), draws.data_ptr(), B, N, int(steps), float(eta), gs,
-                                                      self._problem_array(problems) if problems else None,
-                                                      len(problems) if problems else 0, C.byref(conf) if conf is not None else None,
-                                                      int(cond_start_step), pose.data_ptr(), trail.data_ptr() if want_trail else None,
-                                                      stats.data_ptr() if stats is not None else None, _stream_ptr(self.device)),
-                 "pdb_sample_loop_ddim_guided")
-        return pose, trail, stats
+        return self._device_loop("pdb_sample_loop_ddim_guided", (int(steps), float(eta), gs), z, draws, 1 + k if eta > 0 else 1,
+                                 1 + int(steps), gs, problems, cfg, cond_start_step, want_trail, want_stats)
+
+    @staticmethod
+    def _check_host_buffers(z: np.ndarray, draws: np.ndarray, draw_slots: int, trail_out, trail_slots: int, stats_out, stats_rows: int):
+        """The host arrays of a host-buffer entry against the loop's slot counts (the library trusts their sizes)."""
+        B, N, _ = z.shape
+        want = (draw_slots, B, N, TARGET_DIM)
+        if draws.shape != want or draws.dtype != np.float32 or not draws.flags.c_contiguous:
+            raise ValueError(f"draws must be C-contiguous float32 {want}, got {draws.shape}")
+        if trail_out is not None and trail_out.shape != (trail_slots, B, N, TARGET_DIM):
+            raise ValueError(f"trail_out must be {(trail_slots, B, N, TARGET_DIM)}, got {trail_out.shape}")
+        if stats_out is not None and stats_out.nbytes < stats_rows * B * GGS_STATS_DTYPE.itemsize:
+            raise ValueError(f"stats_out needs {stats_rows * B} records")
 
     def sample_loop_host(self, z: np.ndarray, draws: np.ndarray, problems, cfg, cond_start_step: int,
                          pose_out: np.ndarray, trail_out: Optional[np.ndarray] = None, stats_out: Optional[np.ndarray] = None):
         """Host-buffer entry (numpy float32 arrays, ideally pinned): the end-to-end call bench.py times."""
         B, N, _ = z.shape
+        guided = clamp_guided(cond_start_step) if problems else 0
+        self._check_host_buffers(z, draws, NUM_TIMESTEPS + 1, trail_out, NUM_TIMESTEPS + 1, stats_out, guided)
         if problems:
             self._check_problems(problems, B, N)
         conf = ggs_config_struct(cfg) if problems else None
@@ -772,52 +781,41 @@ class Context:
                                                    _stream_ptr(self.device)), "pdb_sample_loop_host")
         return pose_out
 
+    def _host_matches_loop(self, entry: str, ddim_args, z: np.ndarray, draws: np.ndarray, draw_slots: int, trail_slots: int,
+                           stats_rows: int, matches_dicts, cfg, cond_start_step: int, pose_out, trail_out, stats_out):
+        B, N, _ = z.shape
+        self._check_host_buffers(z, draws, draw_slots, trail_out, trail_slots, stats_out, stats_rows)
+        ptrs, counts, shape, _keep = self._host_match_arrays(matches_dicts, B, N)
+        conf = ggs_config_struct(cfg)
+        with torch.cuda.device(self.device):
+            rc = getattr(self.lib, entry)(self.handle, z.ctypes.data, draws.ctypes.data, B, N, *ddim_args, ptrs[0], ptrs[1], ptrs[2],
+                                          counts, shape[0], shape[1], C.byref(conf), int(cond_start_step), pose_out.ctypes.data,
+                                          trail_out.ctypes.data if trail_out is not None else None,
+                                          stats_out.ctypes.data if stats_out is not None else None, _stream_ptr(self.device))
+        if rc == -1:
+            raise ValueError(self.lib.pdb_last_error(self.handle).decode())
+        self._ok(rc, entry)
+        return pose_out
+
     def sample_loop_host_matches(self, z: np.ndarray, draws: np.ndarray, matches_dicts, cfg, cond_start_step: int,
                                  pose_out: np.ndarray, trail_out: Optional[np.ndarray] = None, stats_out: Optional[np.ndarray] = None):
         """The end-to-end call from the reference's matches_dict format (one dict per sequence): the match sets are packed and
         uploaded while the unguided steps already run (pdb_sample_loop_host_matches)."""
-        B, N, _ = z.shape
-        ptrs, counts, shape, _keep = self._host_match_arrays(matches_dicts, B, N)
-        conf = ggs_config_struct(cfg)
-        with torch.cuda.device(self.device):
-            rc = self.lib.pdb_sample_loop_host_matches(self.handle, z.ctypes.data, draws.ctypes.data, B, N, ptrs[0], ptrs[1], ptrs[2],
-                                                       counts, shape[0], shape[1], C.byref(conf), int(cond_start_step),
-                                                       pose_out.ctypes.data, trail_out.ctypes.data if trail_out is not None else None,
-                                                       stats_out.ctypes.data if stats_out is not None else None,
-                                                       _stream_ptr(self.device))
-        if rc == -1:
-            raise ValueError(self.lib.pdb_last_error(self.handle).decode())
-        self._ok(rc, "pdb_sample_loop_host_matches")
-        return pose_out
+        return self._host_matches_loop("pdb_sample_loop_host_matches", (), z, draws, NUM_TIMESTEPS + 1, NUM_TIMESTEPS + 1,
+                                       clamp_guided(cond_start_step), matches_dicts, cfg, cond_start_step, pose_out, trail_out,
+                                       stats_out)
 
     def sample_loop_host_matches_ddim(self, z: np.ndarray, draws: np.ndarray, matches_dicts, cfg, cond_start_step: int, steps: int,
                                       eta: float, pose_out: np.ndarray, trail_out: Optional[np.ndarray] = None,
                                       stats_out: Optional[np.ndarray] = None, guided_steps: Optional[int] = None):
         """sample_loop_host_matches on the DDIM loop of sample_loop_ddim (pdb_sample_loop_host_matches_ddim): draws [1 + k, B, N, 9]
         for eta > 0, [1, B, N, 9] for eta == 0; trail_out [1 + steps, B, N, 9]; stats_out g' records per sequence."""
-        B, N, _ = z.shape
-        guided = max(0, min(int(cond_start_step), NUM_TIMESTEPS))
+        guided = clamp_guided(cond_start_step)
         k = ddim_check(steps, guided, eta, guided_steps)
         gs = guided if guided_steps is None else int(guided_steps)
-        if draws.shape != (1 + k if eta > 0 else 1, B, N, TARGET_DIM) or draws.dtype != np.float32 or not draws.flags.c_contiguous:
-            raise ValueError(f"draws must be C-contiguous float32 {(1 + k if eta > 0 else 1, B, N, TARGET_DIM)}, got {draws.shape}")
-        if trail_out is not None and trail_out.shape != (1 + int(steps), B, N, TARGET_DIM):
-            raise ValueError(f"trail_out must be {(1 + int(steps), B, N, TARGET_DIM)}, got {trail_out.shape}")
-        if stats_out is not None and stats_out.nbytes < gs * B * GGS_STATS_DTYPE.itemsize:
-            raise ValueError(f"stats_out needs {gs * B} records")
-        ptrs, counts, shape, _keep = self._host_match_arrays(matches_dicts, B, N)
-        conf = ggs_config_struct(cfg)
-        with torch.cuda.device(self.device):
-            rc = self.lib.pdb_sample_loop_host_matches_ddim(self.handle, z.ctypes.data, draws.ctypes.data, B, N, int(steps), float(eta),
-                                                            gs, ptrs[0], ptrs[1], ptrs[2], counts, shape[0], shape[1], C.byref(conf),
-                                                            int(cond_start_step), pose_out.ctypes.data,
-                                                            trail_out.ctypes.data if trail_out is not None else None,
-                                                            stats_out.ctypes.data if stats_out is not None else None,
-                                                            _stream_ptr(self.device))
-        if rc == -1:
-            raise ValueError(self.lib.pdb_last_error(self.handle).decode())
-        self._ok(rc, "pdb_sample_loop_host_matches_ddim")
-        return pose_out
+        return self._host_matches_loop("pdb_sample_loop_host_matches_ddim", (int(steps), float(eta), gs), z, draws,
+                                       1 + k if eta > 0 else 1, 1 + int(steps), gs, matches_dicts, cfg, cond_start_step, pose_out,
+                                       trail_out, stats_out)
 
     @staticmethod
     def _host_match_arrays(matches_dicts, B: int, N: int):

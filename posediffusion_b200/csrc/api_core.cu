@@ -95,6 +95,7 @@ int pdb_create(pdb_context** out, int device_ordinal) {
   Context* ctx = new (std::nothrow) Context();
   if (!ctx) return PDB_ERR_CUDA;
   ctx->device = device_ordinal;
+  ctx->attr = kernel_attrs(device_ordinal, count);
   ctx->sm_count = prop.multiProcessorCount;
   ctx->cc_major = prop.major;
   ctx->cc_minor = prop.minor;
@@ -482,7 +483,7 @@ int launch_ggs_chunk(Context* ctx, const GgsBatch& batch, int nprob, int max_fra
   const bool lean = !kEval && resident && segs_fit && P.xch_mode == 1 && !(lean_env && lean_env[0] == '0');
   const void* kernel = lean ? (const void*)ggs_entry<kEval, kPaired, kProbe, !kEval> : (const void*)ggs_entry<kEval, kPaired, kProbe, false>;
   const size_t smem = fixed + (resident ? (size_t)rounds_per_cta * 512 : (size_t)kRingBytes);
-  size_t& attr_bytes = ctx->attr_ggs[(kEval ? 1 : 0) + (kPaired ? 2 : 0) + (kProbe ? 4 : 0) + (lean ? 8 : 0)];
+  size_t& attr_bytes = ctx->attr->ggs[(kEval ? 1 : 0) + (kPaired ? 2 : 0) + (kProbe ? 4 : 0) + (lean ? 8 : 0)];
   if (smem > attr_bytes) {
     PDB_CUDA(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_bytes = smem;

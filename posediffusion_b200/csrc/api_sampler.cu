@@ -108,7 +108,7 @@ template <int TS, bool kFlag>
 int launch_denoiser(Context* ctx, const DenoiserDev& dev, const DenoiserRun& run, int grid, cudaStream_t st) {
   const size_t smem = denoiser_smem_bytes(TS, run.frames);
   if (smem > ctx->smem_optin) return ctx->fail(PDB_ERR_LIMIT, "denoiser needs %zu B shared memory", smem);
-  size_t& attr_bytes = ctx->attr_den[(kFlag ? 8 : 0) + TS / 4 - 1];  // static shared memory counts against the opt-in limit: ask for what we use
+  size_t& attr_bytes = ctx->attr->den[(kFlag ? 8 : 0) + TS / 4 - 1];  // static shared memory counts against the opt-in limit: ask for what we use
   if (smem > attr_bytes) {
     PDB_CUDA(ctx, cudaFuncSetAttribute(denoiser_kernel<TS, kFlag>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_bytes = smem;
@@ -204,71 +204,6 @@ int enqueue_denoiser(Context* ctx, DenoiserRun run, cudaStream_t st, const Denoi
     case 24: return launch_denoiser<24, false>(ctx, dev, run, grid, st);
     default: return launch_denoiser<32, false>(ctx, dev, run, grid, st);
   }
-}
-
-// The sampling loop in two halves, so that a caller can do host work (match packing) between them while the first half runs:
-// loop_prefix enqueues x_T = draws[0] (gaussian_diffuser.py:289) and the unguided steps t = T-1 .. guide_below in ONE launch,
-// loop_guided the guided steps (denoiser -> posterior mean -> GGS in place).  A DDIM prefix (pdb_sample_loop_ddim_guided) is k
-// steps on tables of virtual timesteps T-1 .. T-k; the guided steps that follow are today's DDPM steps, or g' < g DDIM jumps on
-// virtual timesteps g'-1 .. 0 of the same tables.
-struct LoopState {
-  DenoiserRun run = {};
-  int guide_below = 0;
-  int prefix_steps = 0;  // unguided steps before the guided ones: T - guide_below (DDPM) or k (DDIM); trail slot of guided step / jump i = 1 + prefix_steps + i
-  bool first = true;
-  size_t n = 0;
-  float* pose = nullptr;
-  float* trail = nullptr;
-};
-
-// ddim: NULL for the DDPM loop, else the k-step prefix's tables (make_ddim_tables) and noise_draws its draws (NULL: no noise).
-int loop_prefix(Context* ctx, const float* z_dev, const float* draws_dev, int batch, int frames, int guide_below, float* pose_dev,
-                float* trail_dev, cudaStream_t st, LoopState* loop, const DenoiserDev* ddim = nullptr, int ddim_steps = 0,
-                const float* noise_draws = nullptr) {
-  if (guide_below > kT) guide_below = kT;
-  if (guide_below < 0) guide_below = 0;
-  const int prefix_steps = ddim ? ddim_steps : kT - guide_below;
-  const size_t n = (size_t)batch * frames * kTargetDim;
-  PDB_CUDA(ctx, cudaMemcpyAsync(pose_dev, draws_dev, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
-  if (trail_dev) PDB_CUDA(ctx, cudaMemcpyAsync(trail_dev, draws_dev, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
-  loop->n = n;
-  loop->guide_below = guide_below;
-  loop->prefix_steps = prefix_steps;
-  loop->pose = pose_dev;
-  loop->trail = trail_dev;
-  DenoiserRun& run = loop->run;
-  run.batch = batch; run.frames = frames;
-  run.guide_below = guide_below;
-  run.x = pose_dev; run.z = z_dev; run.draws = ddim ? noise_draws : draws_dev; run.trail = trail_dev;
-  if (prefix_steps > 0) {
-    // DDIM: virtual timesteps T-1 .. T-k, all >= guide_below, so the kernel adds noise (draw slot 1 + i) and writes trail slot 1 + i
-    run.t_hi = kT - 1; run.t_lo = kT - prefix_steps;
-    run.compute_zproj = 1;
-    if (int rc = enqueue_denoiser(ctx, run, st, ddim)) return rc;
-    loop->first = false;
-  }
-  return PDB_OK;
-}
-
-// jumps: NULL for the DDPM steps t = guide_below-1 .. 0, else the tables of make_ddim_tables, whose `jump_count` guided DDIM jumps
-// sit at virtual timesteps jump_count-1 .. 0 (below guide_below: the kernel leaves the mean, no noise, no trail slot).
-int loop_guided(Context* ctx, LoopState* loop, pdb_matches* const* problems, const pdb_ggs_config* cfg, pdb_ggs_stats* stats_dev,
-                cudaStream_t st, const DenoiserDev* jumps = nullptr, int jump_count = 0) {
-  DenoiserRun& run = loop->run;
-  const int steps = jumps ? jump_count : loop->guide_below;
-  for (int t = steps - 1; t >= 0; --t) {
-    const int i = steps - 1 - t;
-    run.t_hi = run.t_lo = t;
-    run.compute_zproj = loop->first ? 1 : 0;
-    loop->first = false;
-    if (int rc = enqueue_denoiser(ctx, run, st, jumps)) return rc;
-    pdb_ggs_stats* stats = stats_dev ? stats_dev + (size_t)i * run.batch : nullptr;
-    if (int rc = enqueue_ggs(ctx, problems, run.batch, run.frames, loop->pose, cfg, stats, st)) return rc;
-    if (loop->trail)
-      PDB_CUDA(ctx, cudaMemcpyAsync(loop->trail + (size_t)(1 + loop->prefix_steps + i) * loop->n, loop->pose, sizeof(float) * loop->n,
-                                    cudaMemcpyDeviceToDevice, st));
-  }
-  return PDB_OK;
 }
 
 // float64 betas (torch.linspace: filled symmetrically from both ends) and their cumulative product
@@ -372,27 +307,193 @@ int make_ddim_tables(Context* ctx, const int32_t* tab_t, const float* tab_coef, 
 
 int clamp_guided(int cond_start_step) { return cond_start_step < 0 ? 0 : (cond_start_step > kT ? kT : cond_start_step); }
 
-// A DDIM loop's step table, computed and checked before anything is enqueued.
-struct DdimPlan {
-  int g = 0;      // guided timesteps: clamp(cond_start_step, 0, T)
-  int k = 0;      // unguided prefix steps
-  int jumps = 0;  // guided DDIM jumps on the step tables; 0 when the tail is the g DDPM steps on the weights' own tables
-  int guided = 0; // denoiser evaluations of the guided tail (g' = jumps, or g)
-  int32_t t[kT];
-  float coef[kT * 8];
+// The match sets of a host-matches entry: the reference's host arrays, one sequence each, packed while the prefix runs.
+struct HostMatches {
+  const double* const* kp1;
+  const double* const* kp2;
+  const int64_t* const* i12;
+  const int64_t* m_total;
+  int height, width;
 };
 
-int ddim_plan(Context* ctx, int steps, double eta, int guided_steps, int cond_start_step, DdimPlan* p) {
-  const int g = clamp_guided(cond_start_step);
-  if (!ddim_table(steps, g, guided_steps, eta, 1e-4, 0.1, p->t, p->coef))
-    return ctx->fail(PDB_ERR_INVALID,
-                     "DDIM: %d denoiser steps, %d of them over %d guided timesteps (the guided tail needs %d .. %d, the unguided prefix "
-                     "1 .. %d) and eta %g (>= 0, finite)",
-                     steps, guided_steps, g, g > 0 ? 1 : 0, g, kT - g, eta);
-  p->g = g;
-  p->k = steps - guided_steps;
-  p->guided = guided_steps;
-  p->jumps = guided_steps < g ? guided_steps : 0;
+// One call of a sampling-loop entry point.  z / draws / pose / trail / stats are device buffers, or host buffers that host_loop
+// stages.  Match sets come packed (`problems`), as host arrays (`pack`), or not at all.
+struct LoopArgs {
+  const float* z;
+  const float* draws;
+  int batch, frames;
+  pdb_matches* const* problems;
+  int n_problems;
+  const HostMatches* pack;
+  const pdb_ggs_config* cfg;
+  int cond_start_step;
+  float* pose;
+  float* trail;
+  pdb_ggs_stats* stats;
+  bool ddim = false;  // the loop of pdb_sample_loop_ddim_guided: `steps` evaluations, the last `guided_steps` the guided tail
+  int steps = 0;
+  double eta = 0.0;
+  int guided_steps = 0;
+};
+
+// The loop as the kernels run it, built and checked by plan_loop before anything is enqueued.  The prefix is ONE launch over
+// timesteps T-1 .. T-prefix_steps: the DDPM steps t = T-1 .. g, or the k DDIM steps at virtual timesteps T-1 .. T-k of the step
+// tables (make_ddim_tables).  The tail takes tail_steps denoiser steps at timesteps tail_steps-1 .. 0, each followed by GGS in
+// place and a copy into trail slot 1 + prefix_steps + i: the g DDPM steps on the weights' own tables (also after a DDIM prefix:
+// the tensor-core engine keys its captured step graph on the table addresses), or g' < g DDIM jumps on the step tables (below
+// guide_below, so the kernel leaves the mean, adds no noise and writes no trail slot).  Not copyable: the descriptors may point
+// at steps_dev.
+struct LoopPlan {
+  LoopPlan() = default;
+  LoopPlan(const LoopPlan&) = delete;
+  int g = 0;                 // guide_below: clamp(cond_start_step, 0, T); 0 for a DDPM loop without match sets
+  int prefix_steps = 0;      // T - g (DDPM, none at g = T) or k (DDIM)
+  int tail_steps = 0;        // g (DDPM) or g' (DDIM) with match sets, else 0
+  const DenoiserDev* prefix_tables = nullptr;
+  const DenoiserDev* tail_tables = nullptr;
+  bool noise = true;         // the kernel adds noise from draws[1 + i] (false: DDIM at eta = 0, whose draws are x_T alone)
+  size_t draw_slots = 0, trail_slots = 0, stats_rows = 0;
+  bool ddim = false;         // DDIM: the step table's rows, its prefix steps k and guided jumps (0: a DDPM tail)
+  int jumps = 0;
+  int32_t t[kT];
+  float coef[kT * 8];
+  DenoiserDev steps_dev;     // the step tables, filled by run_loop
+};
+
+// Every check of a sampling-loop call, made before anything is enqueued.  Only a match set that fails to pack is found later,
+// while the prefix runs (run_loop).
+int plan_loop(Context* ctx, const LoopArgs& a, LoopPlan* p) {
+  const HostMatches* hm = a.pack;
+  if (!a.z || !a.draws || !a.pose || (hm && (!hm->kp1 || !hm->kp2 || !hm->i12 || !hm->m_total || !a.cfg)))
+    return ctx->fail(PDB_ERR_INVALID, "null argument");
+  if (a.batch < 1 || a.frames < 1) return ctx->fail(PDB_ERR_INVALID, "empty batch");
+  if (a.frames > PDB_MAX_FRAMES) return ctx->fail(PDB_ERR_LIMIT, "frames %d > PDB_MAX_FRAMES", a.frames);
+  if (!ctx->weights) return ctx->fail(PDB_ERR_STATE, "denoiser weights not loaded (pdb_denoiser_load)");
+  const bool sets = a.problems || hm;
+  if (sets && !a.cfg) return ctx->fail(PDB_ERR_INVALID, "GGS config missing");
+  if (a.problems) {
+    if (a.n_problems != a.batch)
+      return ctx->fail(PDB_ERR_INVALID, "%d match sets for a batch of %d sequences (one per sequence)", a.n_problems, a.batch);
+    // a set packed for another frame count would stride the pose wrongly
+    if (int rc = check_ggs_problems(ctx, a.problems, a.batch, a.frames)) return rc;
+  }
+  p->g = sets || a.ddim ? clamp_guided(a.cond_start_step) : 0;
+  p->prefix_tables = p->tail_tables = &ctx->weights->dev;
+  p->ddim = a.ddim;
+  if (a.ddim) {
+    if (!ddim_table(a.steps, p->g, a.guided_steps, a.eta, 1e-4, 0.1, p->t, p->coef))
+      return ctx->fail(PDB_ERR_INVALID,
+                       "DDIM: %d denoiser steps, %d of them over %d guided timesteps (the guided tail needs %d .. %d, the unguided "
+                       "prefix 1 .. %d) and eta %g (>= 0, finite)",
+                       a.steps, a.guided_steps, p->g, p->g > 0 ? 1 : 0, p->g, kT - p->g, a.eta);
+    p->prefix_steps = a.steps - a.guided_steps;
+    p->jumps = a.guided_steps < p->g ? a.guided_steps : 0;
+    p->tail_steps = sets ? a.guided_steps : 0;  // without match sets the prefix alone runs: pose = x_{g-1}
+    p->prefix_tables = &p->steps_dev;
+    if (p->jumps) p->tail_tables = &p->steps_dev;
+    p->noise = a.eta > 0.0;
+    p->draw_slots = p->noise ? 1 + p->prefix_steps : 1;
+    p->trail_slots = 1 + a.steps;
+  } else {
+    p->prefix_steps = kT - p->g;
+    p->tail_steps = p->g;
+    p->draw_slots = p->trail_slots = kT + 1;
+  }
+  p->stats_rows = p->tail_steps;
+  if (p->tail_steps && a.cfg->iter_num < 0) return ctx->fail(PDB_ERR_INVALID, "iter_num < 0");
+  return PDB_OK;
+}
+
+// The sampling loop of every entry point, on device buffers: fill the step tables (DDIM), enqueue x_T = draws[0]
+// (gaussian_diffuser.py:289) and the prefix, take the match sets -- given, or packed into `packed` now, while the prefix runs (the
+// caller frees them once the stream is synchronised) -- and enqueue the guided tail.
+int run_loop(Context* ctx, const LoopArgs& a, LoopPlan* p, cudaStream_t st, std::vector<pdb_matches*>* packed) {
+  if (p->ddim)
+    if (int rc = make_ddim_tables(ctx, p->t, p->coef, p->prefix_steps, p->jumps, st, &p->steps_dev)) return rc;
+  const size_t n = (size_t)a.batch * a.frames * kTargetDim;
+  PDB_CUDA(ctx, cudaMemcpyAsync(a.pose, a.draws, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
+  if (a.trail) PDB_CUDA(ctx, cudaMemcpyAsync(a.trail, a.draws, sizeof(float) * n, cudaMemcpyDeviceToDevice, st));
+  DenoiserRun run = {};
+  run.batch = a.batch; run.frames = a.frames;
+  run.guide_below = p->g;
+  run.x = a.pose; run.z = a.z; run.draws = p->noise ? a.draws : nullptr; run.trail = a.trail;
+  run.compute_zproj = 1;
+  if (p->prefix_steps > 0) {
+    run.t_hi = kT - 1; run.t_lo = kT - p->prefix_steps;
+    if (int rc = enqueue_denoiser(ctx, run, st, p->prefix_tables)) return rc;
+    run.compute_zproj = 0;
+  }
+  pdb_matches* const* sets = a.problems;
+  if (const HostMatches* hm = a.pack) {  // pdb_matches_pack returns once ITS stream has taken the upload
+    if (!ctx->pack_stream) PDB_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->pack_stream, cudaStreamNonBlocking));
+    packed->assign((size_t)a.batch, nullptr);
+    for (int b = 0; b < a.batch; ++b)
+      if (int rc = pdb_matches_pack(reinterpret_cast<pdb_context*>(ctx), hm->kp1[b], hm->kp2[b], hm->i12[b], hm->m_total[b], a.frames,
+                                    hm->height, hm->width, 0, ctx->pack_stream, &(*packed)[b]))
+        return rc;
+    sets = packed->data();
+    if (int rc = check_ggs_problems(ctx, sets, a.batch, a.frames)) return rc;
+  }
+  for (int i = 0; i < p->tail_steps; ++i) {
+    run.t_hi = run.t_lo = p->tail_steps - 1 - i;
+    if (int rc = enqueue_denoiser(ctx, run, st, p->tail_tables)) return rc;
+    run.compute_zproj = 0;
+    pdb_ggs_stats* stats = a.stats ? a.stats + (size_t)i * a.batch : nullptr;
+    if (int rc = enqueue_ggs(ctx, sets, a.batch, a.frames, a.pose, a.cfg, stats, st)) return rc;
+    if (a.trail)
+      PDB_CUDA(ctx, cudaMemcpyAsync(a.trail + (size_t)(1 + p->prefix_steps + i) * n, a.pose, sizeof(float) * n,
+                                    cudaMemcpyDeviceToDevice, st));
+  }
+  return PDB_OK;
+}
+
+int device_loop(pdb_context* c, const LoopArgs& a, void* stream) {
+  if (!c) return PDB_ERR_INVALID;
+  Context* ctx = reinterpret_cast<Context*>(c);
+  LoopPlan plan;
+  if (int rc = plan_loop(ctx, a, &plan)) return rc;
+  PDB_CUDA(ctx, cudaSetDevice(ctx->device));
+  return run_loop(ctx, a, &plan, static_cast<cudaStream_t>(stream), nullptr);
+}
+
+// The host-buffer entries: one staging buffer ctx->stage = [z | draws | pose | trail | stats] laid out from the plan's slot counts
+// (separate from pdb_denoiser_forward's use of it, grown on demand), z and the draws copied in, the loop, then pose, trail and
+// stats copied out and the stream synchronised -- on the error path too, before packed match sets are released.
+int host_loop(pdb_context* c, const LoopArgs& h, void* stream) {
+  if (!c) return PDB_ERR_INVALID;
+  Context* ctx = reinterpret_cast<Context*>(c);
+  LoopPlan plan;
+  if (int rc = plan_loop(ctx, h, &plan)) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  PDB_CUDA(ctx, cudaSetDevice(ctx->device));
+  const size_t n = (size_t)h.batch * h.frames * kTargetDim;
+  const size_t f_z = (size_t)h.batch * h.frames * kZ, f_draws = plan.draw_slots * n, f_trail = h.trail ? plan.trail_slots * n : 0;
+  const size_t stats_bytes = h.stats ? sizeof(pdb_ggs_stats) * plan.stats_rows * h.batch : 0;
+  if (int rc = ensure_buffer(ctx, &ctx->stage, &ctx->stage_bytes, sizeof(float) * (f_z + f_draws + n + f_trail) + stats_bytes + 256))
+    return rc;
+  float* z = static_cast<float*>(ctx->stage);
+  float* draws = z + f_z;
+  float* pose = draws + f_draws;
+  LoopArgs d = h;
+  d.z = z; d.draws = draws; d.pose = pose;
+  d.trail = h.trail ? pose + n : nullptr;
+  d.stats = h.stats ? reinterpret_cast<pdb_ggs_stats*>(pose + n + f_trail) : nullptr;
+  PDB_CUDA(ctx, cudaMemcpyAsync(z, h.z, sizeof(float) * f_z, cudaMemcpyHostToDevice, st));
+  PDB_CUDA(ctx, cudaMemcpyAsync(draws, h.draws, sizeof(float) * f_draws, cudaMemcpyHostToDevice, st));
+  if (d.stats) PDB_CUDA(ctx, cudaMemsetAsync(d.stats, 0, stats_bytes, st));
+  std::vector<pdb_matches*> packed;
+  const int rc = run_loop(ctx, d, &plan, st, &packed);
+  cudaError_t err = cudaSuccess;
+  if (rc == PDB_OK) {
+    err = cudaMemcpyAsync(h.pose, pose, sizeof(float) * n, cudaMemcpyDeviceToHost, st);
+    if (err == cudaSuccess && h.trail) err = cudaMemcpyAsync(h.trail, d.trail, sizeof(float) * f_trail, cudaMemcpyDeviceToHost, st);
+    if (err == cudaSuccess && h.stats && stats_bytes) err = cudaMemcpyAsync(h.stats, d.stats, stats_bytes, cudaMemcpyDeviceToHost, st);
+  }
+  const cudaError_t sync = cudaStreamSynchronize(st);
+  for (pdb_matches* m : packed) pdb_matches_free(m);
+  if (rc != PDB_OK) return rc;
+  if (err != cudaSuccess || sync != cudaSuccess)
+    return ctx->fail(PDB_ERR_CUDA, "sample loop failed: %s", cudaGetErrorString(err != cudaSuccess ? err : sync));
   return PDB_OK;
 }
 
@@ -672,19 +773,8 @@ int pdb_p_sample(pdb_context* c, const float* x_dev, int32_t t, const float* z_d
 int pdb_sample_loop(pdb_context* c, const float* z_dev, const float* draws_dev, int32_t batch, int32_t frames,
                     pdb_matches* const* problems, int32_t n_problems, const pdb_ggs_config* cfg, int32_t cond_start_step,
                     float* pose_dev, float* trail_dev, pdb_ggs_stats* stats_dev, void* stream) {
-  if (!c) return PDB_ERR_INVALID;
-  Context* ctx = reinterpret_cast<Context*>(c);
-  if (!z_dev || !draws_dev || !pose_dev) return ctx->fail(PDB_ERR_INVALID, "null argument");
-  if (problems && !cfg) return ctx->fail(PDB_ERR_INVALID, "GGS config missing");
-  if (problems && n_problems != batch)
-    return ctx->fail(PDB_ERR_INVALID, "%d match sets for a batch of %d sequences (one per sequence)", n_problems, batch);
-  if (problems)  // before anything is enqueued: a set packed for another frame count would stride the pose wrongly
-    if (int rc = check_ggs_problems(ctx, problems, batch, frames)) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  PDB_CUDA(ctx, cudaSetDevice(ctx->device));
-  LoopState loop;
-  if (int rc = loop_prefix(ctx, z_dev, draws_dev, batch, frames, problems ? cond_start_step : 0, pose_dev, trail_dev, st, &loop)) return rc;
-  return loop_guided(ctx, &loop, problems, cfg, stats_dev, st);
+  return device_loop(c, {z_dev, draws_dev, batch, frames, problems, n_problems, nullptr, cfg, cond_start_step, pose_dev, trail_dev,
+                         stats_dev}, stream);
 }
 
 int pdb_ddim_table(int32_t steps, int32_t guide_below, double eta, double beta_1, double beta_T, int32_t* t_out, float* coef_out) {
@@ -708,146 +798,28 @@ int pdb_sample_loop_ddim_guided(pdb_context* c, const float* z_dev, const float*
                                 int32_t steps, double eta, int32_t guided_steps, pdb_matches* const* problems, int32_t n_problems,
                                 const pdb_ggs_config* cfg, int32_t cond_start_step, float* pose_dev, float* trail_dev,
                                 pdb_ggs_stats* stats_dev, void* stream) {
-  if (!c) return PDB_ERR_INVALID;
-  Context* ctx = reinterpret_cast<Context*>(c);
-  if (!z_dev || !draws_dev || !pose_dev) return ctx->fail(PDB_ERR_INVALID, "null argument");
-  if (batch < 1 || frames < 1) return ctx->fail(PDB_ERR_INVALID, "empty batch");
-  if (frames > PDB_MAX_FRAMES) return ctx->fail(PDB_ERR_LIMIT, "frames %d > PDB_MAX_FRAMES", frames);
-  if (problems && !cfg) return ctx->fail(PDB_ERR_INVALID, "GGS config missing");
-  if (problems && n_problems != batch)
-    return ctx->fail(PDB_ERR_INVALID, "%d match sets for a batch of %d sequences (one per sequence)", n_problems, batch);
-  DdimPlan plan;
-  if (int rc = ddim_plan(ctx, steps, eta, guided_steps, cond_start_step, &plan)) return rc;
-  if (problems)
-    if (int rc = check_ggs_problems(ctx, problems, batch, frames)) return rc;
-  if (!ctx->weights) return ctx->fail(PDB_ERR_STATE, "denoiser weights not loaded (pdb_denoiser_load)");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  PDB_CUDA(ctx, cudaSetDevice(ctx->device));
-  DenoiserDev tables;
-  if (int rc = make_ddim_tables(ctx, plan.t, plan.coef, plan.k, plan.jumps, st, &tables)) return rc;
-  LoopState loop;
-  if (int rc = loop_prefix(ctx, z_dev, draws_dev, batch, frames, plan.g, pose_dev, trail_dev, st, &loop, &tables, plan.k,
-                           eta > 0.0 ? draws_dev : nullptr))
-    return rc;
-  if (!problems) return PDB_OK;  // cond_start_step > 0 without match sets: the prefix alone, x_{g-1} (generic cond_fn callers)
-  return loop_guided(ctx, &loop, problems, cfg, stats_dev, st, plan.jumps ? &tables : nullptr, plan.jumps);
+  return device_loop(c, {z_dev, draws_dev, batch, frames, problems, n_problems, nullptr, cfg, cond_start_step, pose_dev, trail_dev,
+                         stats_dev, true, steps, eta, guided_steps}, stream);
 }
 
 int pdb_sample_loop_host(pdb_context* c, const float* z_host, const float* draws_host, int32_t batch, int32_t frames,
                          pdb_matches* const* problems, int32_t n_problems, const pdb_ggs_config* cfg, int32_t cond_start_step,
                          float* pose_host, float* trail_host, pdb_ggs_stats* stats_host, void* stream) {
-  if (!c) return PDB_ERR_INVALID;
-  Context* ctx = reinterpret_cast<Context*>(c);
-  if (!z_host || !draws_host || !pose_host) return ctx->fail(PDB_ERR_INVALID, "null argument");
-  if (problems && n_problems != batch)
-    return ctx->fail(PDB_ERR_INVALID, "%d match sets for a batch of %d sequences (one per sequence)", n_problems, batch);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  PDB_CUDA(ctx, cudaSetDevice(ctx->device));
-  const size_t S = (size_t)batch * frames, n = S * kTargetDim;
-  const int guided = problems ? (cond_start_step < 0 ? 0 : (cond_start_step > kT ? kT : cond_start_step)) : 0;
-  const size_t f_z = S * kZ, f_draws = (size_t)(kT + 1) * n, f_pose = n, f_trail = trail_host ? (size_t)(kT + 1) * n : 0;
-  const size_t stats_bytes = stats_host ? sizeof(pdb_ggs_stats) * (size_t)guided * batch : 0;
-  const size_t bytes = sizeof(float) * (f_z + f_draws + f_pose + f_trail) + stats_bytes + 256;
-  // separate staging area from pdb_denoiser_forward's: reuse ctx->stage (grown on demand)
-  if (int rc = ensure_buffer(ctx, &ctx->stage, &ctx->stage_bytes, bytes)) return rc;
-  float* z_dev = static_cast<float*>(ctx->stage);
-  float* draws_dev = z_dev + f_z;
-  float* pose_dev = draws_dev + f_draws;
-  float* trail_dev = trail_host ? pose_dev + f_pose : nullptr;
-  pdb_ggs_stats* stats_dev = stats_host ? reinterpret_cast<pdb_ggs_stats*>(pose_dev + f_pose + f_trail) : nullptr;
-  PDB_CUDA(ctx, cudaMemcpyAsync(z_dev, z_host, sizeof(float) * f_z, cudaMemcpyHostToDevice, st));
-  PDB_CUDA(ctx, cudaMemcpyAsync(draws_dev, draws_host, sizeof(float) * f_draws, cudaMemcpyHostToDevice, st));
-  if (stats_dev) PDB_CUDA(ctx, cudaMemsetAsync(stats_dev, 0, stats_bytes, st));
-  if (int rc = pdb_sample_loop(c, z_dev, draws_dev, batch, frames, problems, n_problems, cfg, cond_start_step, pose_dev, trail_dev,
-                               stats_dev, stream))
-    return rc;
-  PDB_CUDA(ctx, cudaMemcpyAsync(pose_host, pose_dev, sizeof(float) * f_pose, cudaMemcpyDeviceToHost, st));
-  if (trail_host) PDB_CUDA(ctx, cudaMemcpyAsync(trail_host, trail_dev, sizeof(float) * f_trail, cudaMemcpyDeviceToHost, st));
-  if (stats_host && stats_bytes) PDB_CUDA(ctx, cudaMemcpyAsync(stats_host, stats_dev, stats_bytes, cudaMemcpyDeviceToHost, st));
-  PDB_CUDA(ctx, cudaStreamSynchronize(st));
-  return PDB_OK;
+  return host_loop(c, {z_host, draws_host, batch, frames, problems, n_problems, nullptr, cfg, cond_start_step, pose_host, trail_host,
+                       stats_host}, stream);
 }
 
 // The end-to-end call of a guided run that starts from the reference's match format (host arrays, one match set per sequence):
-// the match sets are packed and uploaded WHILE the unguided prefix of the loop (t = T-1 .. cond_start_step, one launch) runs on
-// the GPU -- the packer is host work plus a copy on its own stream, the prefix does not need the matches.  `ddim` NULL: the DDPM
-// loop; else the checked plan of a DDIM loop (pdb_sample_loop_host_matches_ddim).
-static int host_matches_loop(pdb_context* c, const float* z_host, const float* draws_host, int32_t batch, int32_t frames,
-                             const double* const* kp1, const double* const* kp2, const int64_t* const* i12, const int64_t* m_total,
-                             int32_t height, int32_t width, const pdb_ggs_config* cfg, int32_t cond_start_step, float* pose_host,
-                             float* trail_host, pdb_ggs_stats* stats_host, void* stream, const DdimPlan* ddim, double eta) {
-  Context* ctx = reinterpret_cast<Context*>(c);
-  if (ddim && !ctx->weights) return ctx->fail(PDB_ERR_STATE, "denoiser weights not loaded (pdb_denoiser_load)");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  PDB_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (!ctx->pack_stream) PDB_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->pack_stream, cudaStreamNonBlocking));
-  const size_t S = (size_t)batch * frames, n = S * kTargetDim;
-  const int guided = ddim ? ddim->guided : clamp_guided(cond_start_step);
-  const size_t draw_slots = ddim ? (eta > 0.0 ? 1 + ddim->k : 1) : kT + 1, trail_slots = ddim ? 1 + ddim->k + ddim->guided : kT + 1;
-  const size_t f_z = S * kZ, f_draws = draw_slots * n, f_pose = n, f_trail = trail_host ? trail_slots * n : 0;
-  const size_t stats_bytes = stats_host ? sizeof(pdb_ggs_stats) * (size_t)guided * batch : 0;
-  const size_t bytes = sizeof(float) * (f_z + f_draws + f_pose + f_trail) + stats_bytes + 256;
-  if (int rc = ensure_buffer(ctx, &ctx->stage, &ctx->stage_bytes, bytes)) return rc;
-  float* z_dev = static_cast<float*>(ctx->stage);
-  float* draws_dev = z_dev + f_z;
-  float* pose_dev = draws_dev + f_draws;
-  float* trail_dev = trail_host ? pose_dev + f_pose : nullptr;
-  pdb_ggs_stats* stats_dev = stats_host ? reinterpret_cast<pdb_ggs_stats*>(pose_dev + f_pose + f_trail) : nullptr;
-  PDB_CUDA(ctx, cudaMemcpyAsync(z_dev, z_host, sizeof(float) * f_z, cudaMemcpyHostToDevice, st));
-  PDB_CUDA(ctx, cudaMemcpyAsync(draws_dev, draws_host, sizeof(float) * f_draws, cudaMemcpyHostToDevice, st));
-  if (stats_dev) PDB_CUDA(ctx, cudaMemsetAsync(stats_dev, 0, stats_bytes, st));
-  LoopState loop;
-  DenoiserDev tables;
-  if (ddim) {
-    if (int rc = make_ddim_tables(ctx, ddim->t, ddim->coef, ddim->k, ddim->jumps, st, &tables)) return rc;
-    if (int rc = loop_prefix(ctx, z_dev, draws_dev, batch, frames, ddim->g, pose_dev, trail_dev, st, &loop, &tables, ddim->k,
-                             eta > 0.0 ? draws_dev : nullptr))
-      return rc;
-  } else if (int rc = loop_prefix(ctx, z_dev, draws_dev, batch, frames, guided, pose_dev, trail_dev, st, &loop)) {
-    return rc;
-  }
-  // ---- host: pack while the prefix runs (pdb_matches_pack returns once ITS stream has taken the upload) ----
-  std::vector<pdb_matches*> sets((size_t)batch, nullptr);
-  int rc = PDB_OK;
-  for (int b = 0; b < batch && rc == PDB_OK; ++b)
-    rc = pdb_matches_pack(c, kp1[b], kp2[b], i12[b], m_total[b], frames, height, width, 0, ctx->pack_stream, &sets[b]);
-  if (rc == PDB_OK) rc = check_ggs_problems(ctx, sets.data(), batch, frames);
-  const bool jumps = ddim && ddim->jumps;
-  if (rc == PDB_OK) rc = loop_guided(ctx, &loop, sets.data(), cfg, stats_dev, st, jumps ? &tables : nullptr, jumps ? ddim->jumps : 0);
-  cudaError_t err = cudaSuccess;
-  if (rc == PDB_OK) {
-    err = cudaMemcpyAsync(pose_host, pose_dev, sizeof(float) * f_pose, cudaMemcpyDeviceToHost, st);
-    if (err == cudaSuccess && trail_host) err = cudaMemcpyAsync(trail_host, trail_dev, sizeof(float) * f_trail, cudaMemcpyDeviceToHost, st);
-    if (err == cudaSuccess && stats_host && stats_bytes)
-      err = cudaMemcpyAsync(stats_host, stats_dev, stats_bytes, cudaMemcpyDeviceToHost, st);
-  }
-  const cudaError_t sync = cudaStreamSynchronize(st);  // also on the error path: the match sets are released below
-  for (pdb_matches* m : sets) pdb_matches_free(m);
-  if (rc != PDB_OK) return rc;
-  if (err != cudaSuccess || sync != cudaSuccess)
-    return ctx->fail(PDB_ERR_CUDA, "sample loop failed: %s", cudaGetErrorString(err != cudaSuccess ? err : sync));
-  return PDB_OK;
-}
-
-static int host_matches_check(pdb_context* c, const float* z_host, const float* draws_host, int32_t batch, int32_t frames,
-                              const double* const* kp1, const double* const* kp2, const int64_t* const* i12, const int64_t* m_total,
-                              const pdb_ggs_config* cfg, const float* pose_host) {
-  Context* ctx = reinterpret_cast<Context*>(c);
-  if (!z_host || !draws_host || !pose_host || !kp1 || !kp2 || !i12 || !m_total || !cfg)
-    return ctx->fail(PDB_ERR_INVALID, "null argument");
-  if (batch < 1 || frames < 1) return ctx->fail(PDB_ERR_INVALID, "bad batch / frames");
-  return PDB_OK;
-}
-
+// the match sets are packed and uploaded WHILE the unguided prefix of the loop runs on the GPU -- the packer is host work plus a
+// copy on its own stream, the prefix does not need the matches.
 int pdb_sample_loop_host_matches(pdb_context* c, const float* z_host, const float* draws_host, int32_t batch, int32_t frames,
                                  const double* const* kp1, const double* const* kp2, const int64_t* const* i12,
                                  const int64_t* m_total, int32_t height, int32_t width, const pdb_ggs_config* cfg,
                                  int32_t cond_start_step, float* pose_host, float* trail_host, pdb_ggs_stats* stats_host,
                                  void* stream) {
-  if (!c) return PDB_ERR_INVALID;
-  if (int rc = host_matches_check(c, z_host, draws_host, batch, frames, kp1, kp2, i12, m_total, cfg, pose_host)) return rc;
-  return host_matches_loop(c, z_host, draws_host, batch, frames, kp1, kp2, i12, m_total, height, width, cfg, cond_start_step,
-                           pose_host, trail_host, stats_host, stream, nullptr, 0.0);
+  const HostMatches hm = {kp1, kp2, i12, m_total, height, width};
+  return host_loop(c, {z_host, draws_host, batch, frames, nullptr, batch, &hm, cfg, cond_start_step, pose_host, trail_host,
+                       stats_host}, stream);
 }
 
 int pdb_sample_loop_host_matches_ddim(pdb_context* c, const float* z_host, const float* draws_host, int32_t batch, int32_t frames,
@@ -855,14 +827,9 @@ int pdb_sample_loop_host_matches_ddim(pdb_context* c, const float* z_host, const
                                       const double* const* kp2, const int64_t* const* i12, const int64_t* m_total, int32_t height,
                                       int32_t width, const pdb_ggs_config* cfg, int32_t cond_start_step, float* pose_host,
                                       float* trail_host, pdb_ggs_stats* stats_host, void* stream) {
-  if (!c) return PDB_ERR_INVALID;
-  Context* ctx = reinterpret_cast<Context*>(c);
-  if (int rc = host_matches_check(c, z_host, draws_host, batch, frames, kp1, kp2, i12, m_total, cfg, pose_host)) return rc;
-  if (frames > PDB_MAX_FRAMES) return ctx->fail(PDB_ERR_LIMIT, "frames %d > PDB_MAX_FRAMES", frames);
-  DdimPlan plan;
-  if (int rc = ddim_plan(ctx, steps, eta, guided_steps, cond_start_step, &plan)) return rc;
-  return host_matches_loop(c, z_host, draws_host, batch, frames, kp1, kp2, i12, m_total, height, width, cfg, cond_start_step,
-                           pose_host, trail_host, stats_host, stream, &plan, eta);
+  const HostMatches hm = {kp1, kp2, i12, m_total, height, width};
+  return host_loop(c, {z_host, draws_host, batch, frames, nullptr, batch, &hm, cfg, cond_start_step, pose_host, trail_host,
+                       stats_host, true, steps, eta, guided_steps}, stream);
 }
 
 }  // extern "C"

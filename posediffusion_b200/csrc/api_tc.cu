@@ -133,9 +133,9 @@ int enqueue_tc_linear(Context* ctx, const float* X, const float* W, TcEpilogue E
   if (tc_linear_swapped(ctx, E.S, E.O)) {
     E.splits = 1;
     E.stats = 0;
-    if (E.S <= 32) return launch_tc_linear_swap<32>(ctx, X, W, E, ctx->attr_tc_swap[0], st);
-    if (E.S <= 64) return launch_tc_linear_swap<64>(ctx, X, W, E, ctx->attr_tc_swap[1], st);
-    return launch_tc_linear_swap<96>(ctx, X, W, E, ctx->attr_tc_swap[2], st);
+    if (E.S <= 32) return launch_tc_linear_swap<32>(ctx, X, W, E, ctx->attr->tc_swap[0], st);
+    if (E.S <= 64) return launch_tc_linear_swap<64>(ctx, X, W, E, ctx->attr->tc_swap[1], st);
+    return launch_tc_linear_swap<96>(ctx, X, W, E, ctx->attr->tc_swap[2], st);
   }
   const long long wide_tiles = (long long)(E.O / 128) * ((E.S + kTcBM - 1) / kTcBM);
   if (E.O % 128 == 0 && wide_tiles >= ctx->sm_count) {
@@ -143,7 +143,7 @@ int enqueue_tc_linear(Context* ctx, const float* X, const float* W, TcEpilogue E
     // tile ahead while the consumers are in the epilogue
     E.splits = 1;
     E.stats = 0;
-    return launch_tc_linear<128, 6>(ctx, X, W, E, ctx->attr_tc128, st);
+    return launch_tc_linear<128, 6>(ctx, X, W, E, ctx->attr->tc128, st);
   }
   if (E.allow_small && tc_linear_small(ctx, E.S, E.O)) {
     // Fewer 64-feature tiles than SMs (the denoiser at a few hundred tokens): a CTA's k-loop is a serial chain of TMA round
@@ -160,11 +160,11 @@ int enqueue_tc_linear(Context* ctx, const float* X, const float* W, TcEpilogue E
           break;
         }
     if (!E.colsum || E.splits != 1) E.stats = 0;
-    return launch_tc_linear<64, 8>(ctx, X, W, E, ctx->attr_tc_deep, st);
+    return launch_tc_linear<64, 8>(ctx, X, W, E, ctx->attr->tc_deep, st);
   }
   E.splits = 1;
   E.stats = 0;
-  return launch_tc_linear<64, kTcStages>(ctx, X, W, E, ctx->attr_tc, st);
+  return launch_tc_linear<64, kTcStages>(ctx, X, W, E, ctx->attr->tc, st);
 }
 
 // the launcher's "small problem" regime (see above); callers that want in-kernel LayerNorm statistics ask first
@@ -309,7 +309,7 @@ int enqueue_denoiser_tc(Context* ctx, const DenoiserDev& dev, DenoiserRun run, c
     return enqueue_tc_linear(ctx, X, Wm, E, s);
   };
   const size_t att_smem = sizeof(float) * ((size_t)N * (kHD + 4) + (size_t)N * kHD + 2 * kDenWarps * kHD) + 64;
-  size_t& att_attr = ctx->attr_att;
+  size_t& att_attr = ctx->attr->att;
   if (att_smem > att_attr) {
     PDB_CUDA(ctx, cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)att_smem));
     att_attr = att_smem;

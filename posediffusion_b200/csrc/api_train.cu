@@ -90,10 +90,10 @@ size_t attn_fwd_smem(int N) { return sizeof(float) * ((size_t)2 * N * 129 + 8 * 
 size_t attn_bwd_smem(int N) { return sizeof(float) * ((size_t)4 * N * 129 + (size_t)2 * N * (N + 1)); }
 
 int set_attn_smem(Context* ctx) {
-  if (!ctx->attr_train_att) {
+  if (!ctx->attr->train_att) {
     PDB_CUDA(ctx, cudaFuncSetAttribute(train_attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_fwd_smem(kTrainMaxFrames)));
     PDB_CUDA(ctx, cudaFuncSetAttribute(train_attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_bwd_smem(kTrainMaxFrames)));
-    ctx->attr_train_att = true;
+    ctx->attr->train_att = true;
   }
   return PDB_OK;
 }

@@ -163,7 +163,7 @@ extern "C" int pdb_extract_features(pdb_context* c, const float* images_dev, int
     const VitLayer& L = w->layer[l];
     vit_row_stats_kernel<<<(S + 7) / 8, 256, 0, st>>>(X, mean, rstd, S);
     if ((rc = lin(X, L.wqkv, 3 * kVitDim, kVitDim, L.bias_qkv, nullptr, L.colsum_qkv, QKV, 0))) break;
-    if ((rc = enqueue_vit_attention(ctx, QKV, ATT, att_args, ctx->attr_vit_att[0], st))) break;
+    if ((rc = enqueue_vit_attention(ctx, QKV, ATT, att_args, ctx->attr->vit_att[0], st))) break;
     if ((rc = lin(ATT, L.wproj, kVitDim, kVitDim, L.bproj, X, nullptr, X, 0))) break;
     vit_row_stats_kernel<<<(S + 7) / 8, 256, 0, st>>>(X, mean, rstd, S);
     if ((rc = lin(X, L.wfc1, kVitMlp, kVitDim, L.bias_fc1, nullptr, L.colsum_fc1, HID, 1))) break;

@@ -136,7 +136,7 @@ extern "C" int pdb_vit_train_forward(pdb_context* c, const float* const* tensors
     train_launch(ctx, st, train_ln_fwd_kernel<kVitDim>, blocks(S, 8), 256, 0, ws + L.hin[l], W(b + 0), W(b + 1), S, kVitLnEps, ws + L.LNA,
                  ws + L.st1[l]);
     if (int rc = train_gemm(ctx, ws + L.LNA, W(b + 2), W(b + 3), nullptr, ws + L.qkv[l], S, 3 * kVitDim, kVitDim, 0, st)) return rc;
-    if (int rc = enqueue_vit_attention(ctx, ws + L.qkv[l], ws + L.att[l], att_args, ctx->attr_vit_att[1], st)) return rc;
+    if (int rc = enqueue_vit_attention(ctx, ws + L.qkv[l], ws + L.att[l], att_args, ctx->attr->vit_att[1], st)) return rc;
     ctx->launches += 1;  // enqueue_vit_attention leaves its one launch to the caller to count
     if (int rc = train_gemm(ctx, ws + L.att[l], W(b + 4), W(b + 5), ws + L.hin[l], ws + L.hmid[l], S, kVitDim, kVitDim, 0, st)) return rc;
     train_launch(ctx, st, train_ln_fwd_kernel<kVitDim>, blocks(S, 8), 256, 0, ws + L.hmid[l], W(b + 6), W(b + 7), S, kVitLnEps, ws + L.LNA,
@@ -178,9 +178,9 @@ extern "C" int pdb_vit_backward(pdb_context* c, const float* const* tensors, voi
   float *LNA = ws + L.LNA, *D0 = ws + L.D0, *D1 = ws + L.D1, *G1 = ws + L.G1, *PR = ws + L.PR, *H = ws + L.H, *G2 = ws + L.G2;
   const LinearGrad lin = {ctx, S, L.Sp, ws + L.T1, ws + L.T2, ws + L.Wt, ws + L.part, st};
   const size_t att_smem = vit_attn_bwd_smem(kVitMaxTokens);
-  if (ctx->attr_vit_att_bwd < att_smem) {
+  if (ctx->attr->vit_att_bwd < att_smem) {
     PDB_CUDA(ctx, cudaFuncSetAttribute(vit_attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)att_smem));
-    ctx->attr_vit_att_bwd = att_smem;
+    ctx->attr->vit_att_bwd = att_smem;
   }
   // ---- head: only the class rows of the last residual stream receive gradient ----
   const int nb = 4 + 12 * kVitDepth;

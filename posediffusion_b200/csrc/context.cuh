@@ -14,6 +14,24 @@ namespace pdb {
 struct DenoiserWeights;  // denoiser.cuh
 struct VitWeights;       // api_vit.cu
 
+// cudaFuncSetAttribute is per device, not per context: the dynamic shared memory already requested for each kernel, kept once
+// per device so that every context on it sees what the others asked for (a second context must not lower a size a first one
+// launches with).
+struct KernelAttrs {
+  size_t ggs[16] = {}, den[16] = {}, att = 0;
+  bool tc = false, tc128 = false, tc_deep = false;
+  bool tc_swap[3] = {false, false, false};  // swap-AB instantiations (32 / 64 / 96 tokens on the N side)
+  size_t vit_att[2] = {0, 0};  // the forward attention kernel's copy in api_vit.cu / api_vit_train.cu
+  size_t vit_att_bwd = 0;      // backbone attention backward (csrc/api_vit_train.cu)
+  bool train_att = false;      // denoiser training attention, forward and backward (csrc/api_train.cu)
+};
+
+// device < device_count (the process's cudaGetDeviceCount)
+inline KernelAttrs* kernel_attrs(int device, int device_count) {
+  static std::vector<KernelAttrs> per_device((size_t)device_count);
+  return &per_device[(size_t)device];
+}
+
 struct Context {
   int device = -1;
   int sm_count = 0;
@@ -48,19 +66,13 @@ struct Context {
   cudaStream_t tc_capture_stream = nullptr;
   cudaStream_t pack_stream = nullptr;  // match uploads of pdb_sample_loop_host_matches (overlap the unguided prefix)
   int tc_graph_nodes = 0;
-  // cudaFuncSetAttribute is per device: remember per context (= per device) what was already requested
-  size_t attr_ggs[16] = {}, attr_den[16] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0}, attr_att = 0;
-  bool attr_tc = false, attr_tc128 = false, attr_tc_deep = false;
+  KernelAttrs* attr = nullptr;  // kernel_attrs(device)
   bool tc_pdl = true;  // programmatic dependent launch between the kernels of the tensor-core engine's step graph (PDB_TC_PDL=0: off)
   bool tc_swap = false;     // swap-AB tensor-core tiles for <= 96 tokens (pdb_debug_tc_swap); default off
-  bool attr_tc_swap[3] = {false, false, false};  // swap-AB instantiations (32 / 64 / 96 tokens on the N side)
   // image feature extractor (csrc/api_vit.cu)
   VitWeights* vit = nullptr;
   void* vit_ws = nullptr;
   size_t vit_ws_bytes = 0;
-  size_t attr_vit_att[2] = {0, 0};  // the forward attention kernel's copy in api_vit.cu / api_vit_train.cu
-  size_t attr_vit_att_bwd = 0;      // backbone attention backward (csrc/api_vit_train.cu)
-  bool attr_train_att = false;      // denoiser training attention, forward and backward (csrc/api_train.cu)
   int ggs_layout = 1;       // stream layout of match sets packed on this context (ggs_layout.cuh): 0 plain, 1 paired (default)
   int denoiser_engine = 0;  // 0 auto, 1 fp32 persistent kernel, 2 wgmma/TMA tiles (TF32)
   // optional per-kernel timing (bench.py roofline): event pairs per launch, kind 0 = GGS, 1 = denoiser

@@ -412,7 +412,7 @@ __global__ void __launch_bounds__(kAttThreads, 2) vit_attention_kernel(const flo
   }
 }
 // one launch for all scales; shared memory is sized by the longest sequence
-// `attr` is the including translation unit's slot of Context::attr_vit_att (each owns its copy of the kernel)
+// `attr` is the including translation unit's slot of KernelAttrs::vit_att (each owns its copy of the kernel)
 int enqueue_vit_attention(Context* ctx, const float* qkv, float* att, const VitAttArgs& A, size_t& attr, cudaStream_t st) {
   const size_t smem = vit_att_smem_bytes(A.max_tiles);
   if (attr < smem) {

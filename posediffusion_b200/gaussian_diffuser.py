@@ -127,18 +127,10 @@ class GaussianDiffusion(nn.Module):
         if draws is None:
             draws = self.draw_noise(tuple(shape), device, guided_below)
         if fused:
-            problems = cfg = None
-            if cond_fn is not None:
-                cfg = cond_fn.keywords["GGS_cfg"]
-                problems = packed_matches(ctx, cond_fn.keywords["matches_dict"])
-            pose, trail, stats = ctx.sample_loop(z, draws.contiguous(), problems, cfg, cond_start_step)
-            self.last_ggs_stats = stats
-            if stats is not None and bool(cfg.get("verbose", True)):
-                rows = _native.stats_to_numpy(stats).reshape(-1, shape[0])
-                for i, per_step in enumerate(rows):
-                    for row in per_step:
-                        print("\n".join(format_log(min(cond_start_step, self.num_timesteps) - 1 - i, row)))
-            return pose, trail
+            g = _native.clamp_guided(cond_start_step)
+            draws = draws.contiguous()
+            return self._fused_loop(ctx, lambda problems, cfg: ctx.sample_loop(z, draws, problems, cfg, cond_start_step), cond_fn,
+                                    shape[0], g, g)
         # generic cond_fn: Python loop around the native step
         pose = draws[0].clone()
         trail = [pose.unsqueeze(0)]
@@ -149,6 +141,24 @@ class GaussianDiffusion(nn.Module):
             pose = cond_fn(mean, t) if guided else pred
             trail.append(pose.unsqueeze(0))
         return pose, torch.cat(trail)
+
+    def _fused_loop(self, ctx, loop, cond_fn, batch: int, g: int, gs: int):
+        """(pose, trail) of loop(problems, cfg), a native loop over g guided timesteps in gs guided steps, with cond_fn's (the GGS
+        `partial`'s, or None) match sets packed and config.  Keeps the GGS statistics in `last_ggs_stats` and, when GGS_cfg asks
+        for it, prints them under the real timestep each guided step starts from."""
+        problems = cfg = None
+        if cond_fn is not None:
+            cfg = cond_fn.keywords["GGS_cfg"]
+            problems = packed_matches(ctx, cond_fn.keywords["matches_dict"])
+        pose, trail, stats = loop(problems, cfg)
+        self.last_ggs_stats = stats
+        if stats is not None and bool(cfg.get("verbose", True)):
+            starts = _native.guided_times(g, gs)[:0:-1]
+            rows = _native.stats_to_numpy(stats).reshape(-1, batch)
+            for i, per_step in enumerate(rows):
+                for row in per_step:
+                    print("\n".join(format_log(starts[i], row)))
+        return pose, trail
 
     def _fused(self, cond_fn) -> bool:
         return cond_fn is None or (
@@ -180,7 +190,7 @@ class GaussianDiffusion(nn.Module):
         `ddim_draws` makes them."""
         self._require_native()
         steps = self.sampling_timesteps if sampling_timesteps is None else int(sampling_timesteps)
-        guided = max(0, min(int(cond_start_step), self.num_timesteps)) if cond_fn is not None else 0
+        guided = _native.clamp_guided(cond_start_step) if cond_fn is not None else 0
         eta = float(eta)
         k = _native.ddim_check(steps, guided, eta, guided_steps)
         gs = guided if guided_steps is None else int(guided_steps)
@@ -191,19 +201,9 @@ class GaussianDiffusion(nn.Module):
             draws = self.ddim_draws(tuple(shape), device, k, eta)
         draws = draws.contiguous()
         if self._fused(cond_fn):
-            problems = cfg = None
-            if cond_fn is not None:
-                cfg = cond_fn.keywords["GGS_cfg"]
-                problems = packed_matches(ctx, cond_fn.keywords["matches_dict"])
-            pose, trail, stats = ctx.sample_loop_ddim(z, draws, steps, eta, problems, cfg, guided, guided_steps=guided_steps)
-            self.last_ggs_stats = stats
-            if stats is not None and bool(cfg.get("verbose", True)):
-                starts = _native.guided_times(guided, gs)[:0:-1] if gs else []  # the real timestep each guided step starts from
-                rows = _native.stats_to_numpy(stats).reshape(-1, shape[0])
-                for i, per_step in enumerate(rows):
-                    for row in per_step:
-                        print("\n".join(format_log(starts[i], row)))
-            return pose, trail
+            return self._fused_loop(ctx, lambda problems, cfg: ctx.sample_loop_ddim(z, draws, steps, eta, problems, cfg, guided,
+                                                                                   guided_steps=guided_steps),
+                                    cond_fn, shape[0], guided, gs)
         # generic cond_fn: the DDIM prefix natively (it stops at x_{g-1}), then the guided steps around the native step
         pose, trail, _ = ctx.sample_loop_ddim(z, draws, steps, eta, None, None, guided, guided_steps=guided_steps)
         if gs == guided:  # DDPM steps
