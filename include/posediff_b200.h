@@ -371,6 +371,19 @@ int pdb_train_backward(pdb_context* ctx, const float* const* params, void* works
  * gradients do not depend on whether grad_z_dev is given. */
 int pdb_train_backward_z(pdb_context* ctx, const float* const* params, void* workspace, const float* grad_loss_dev, const float* grad_x0_dev,
                          float* const* grads, float* grad_z_dev, void* stream);
+/* Denoiser.forward with a backward (models/denoiser.py:53-76 under autograd): the same engine, workspace size and dropout rule as
+ * the p_losses pair above.  eps_dev [B,N,9] = Denoiser(x_dev [B,N,9], t_dev[b] (int32 [B], one timestep per sequence), z_dev
+ * [B,N,384]) with the activations saved in the workspace.  Timesteps outside [0,100) are handled as in pdb_train_forward.  The
+ * workspace header records which forward filled it: pdb_train_backward[_z] refuses a pdb_denoiser_grad_forward workspace with
+ * PDB_ERR_STATE, and pdb_denoiser_grad_backward a pdb_train_forward one. */
+int pdb_denoiser_grad_forward(pdb_context* ctx, const float* const* params, const float* x_dev, const int32_t* t_dev, const float* z_dev,
+                              int32_t batch, int32_t frames, float dropout_p, uint64_t seed, void* workspace, float* eps_dev, void* stream);
+/* From grad_eps_dev [B,N,9] = dL/deps: grads[108] are overwritten with dL/d params (grads NULL: no parameter gradient, and only the
+ * input-gradient chain runs: no weight, bias, _first or time-MLP gradient kernel), grad_x_dev [B,N,9] with dL/dx (through the
+ * harmonic embedding and the raw pose columns of _first), grad_z_dev [B,N,384] with dL/dz; either may be NULL, but not all three.
+ * Synchronises the stream once to read the workspace header.  Bit-reproducible: no floating-point atomics. */
+int pdb_denoiser_grad_backward(pdb_context* ctx, const float* const* params, void* workspace, const float* grad_eps_dev,
+                               float* const* grads, float* grad_x_dev, float* grad_z_dev, void* stream);
 /* camera_to_pose_encoding, "absT_quaR_logFL" (util/camera_transform.py:108-129): R [count,3,3], T [count,3], focal [count,2] ->
  * pose [count,9] = T | matrix_to_quaternion(R) with the real part made non-negative | log(clamp(focal, min, max)) - bias. */
 int pdb_camera_to_pose(pdb_context* ctx, const float* R_dev, const float* T_dev, const float* focal_dev, int32_t count,

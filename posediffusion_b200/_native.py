@@ -117,6 +117,10 @@ EXPORTS = {
     "pdb_train_backward": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p]),
     "pdb_train_backward_z": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p,
                                        C.c_void_p]),
+    "pdb_denoiser_grad_forward": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                            C.c_float, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "pdb_denoiser_grad_backward": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p,
+                                             C.c_void_p, C.c_void_p]),
     "pdb_vit_train_workspace_bytes": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_double), C.c_int32]),
     "pdb_vit_train_forward": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_double),
                                         C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -465,6 +469,43 @@ class Context:
                 _check_dev(grad_z, "grad_z", self.device)
                 self._ok(self.lib.pdb_train_backward_z(self.handle, arr, ws.data_ptr(), gl, gx, garr, grad_z.data_ptr(),
                                                        _stream_ptr(self.device)), "pdb_train_backward_z")
+        return grads
+
+    def denoiser_grad_forward(self, params: Sequence[torch.Tensor], x, t, z, dropout_p: float, seed: int):
+        """Denoiser.forward on the training engine with one timestep per sequence: returns (workspace, eps).  The workspace holds
+        what denoiser_grad_backward needs; it belongs to the caller (one per outstanding forward)."""
+        B, N, _ = x.shape
+        for name, v, shape in (("x", x, (B, N, TARGET_DIM)), ("z", z, (B, N, Z_DIM))):
+            _check_dev(v, name, self.device, shape)
+        if t.dtype != torch.int32 or tuple(t.shape) != (B,) or t.device != self.device or not t.is_contiguous():
+            raise NativeError(f"t must be a contiguous int32 [{B}] tensor on {self.device}")
+        if N > TRAIN_MAX_FRAMES:
+            raise NativeError(f"the differentiable denoiser supports at most {TRAIN_MAX_FRAMES} frames per sequence, got {N}")
+        ws = torch.empty(train_workspace_bytes(B, N) // 4, dtype=torch.float32, device=self.device)
+        eps = torch.empty_like(x)
+        arr = self._tensor_array(params, PDB_NUM_WEIGHT_TENSORS, "parameter")
+        with torch.cuda.device(self.device):
+            self._ok(self.lib.pdb_denoiser_grad_forward(self.handle, arr, x.data_ptr(), t.data_ptr(), z.data_ptr(), B, N, float(dropout_p),
+                                                        int(seed) & (2**64 - 1), ws.data_ptr(), eps.data_ptr(), _stream_ptr(self.device)),
+                     "pdb_denoiser_grad_forward")
+        return ws, eps
+
+    def denoiser_grad_backward(self, params: Sequence[torch.Tensor], ws: torch.Tensor, grad_eps: torch.Tensor, want_params: bool,
+                               grad_x: Optional[torch.Tensor] = None, grad_z: Optional[torch.Tensor] = None) -> Optional[List[torch.Tensor]]:
+        """From dL/deps: the 108 parameter gradients when `want_params` (else None: only the input-gradient chain runs), and dL/dx
+        / dL/dz written into `grad_x` [B,N,9] / `grad_z` [B,N,384] when given."""
+        arr = self._tensor_array(params, PDB_NUM_WEIGHT_TENSORS, "parameter")
+        _check_dev(grad_eps, "grad_eps", self.device)
+        grads = [torch.empty_like(p) for p in params] if want_params else None
+        garr = (C.c_void_p * len(grads))(*[C.c_void_p(g.data_ptr()) for g in grads]) if want_params else None
+        for name, v in (("grad_x", grad_x), ("grad_z", grad_z)):
+            if v is not None:
+                _check_dev(v, name, self.device)
+        with torch.cuda.device(self.device):
+            self._ok(self.lib.pdb_denoiser_grad_backward(self.handle, arr, ws.data_ptr(), grad_eps.data_ptr(), garr,
+                                                         grad_x.data_ptr() if grad_x is not None else None,
+                                                         grad_z.data_ptr() if grad_z is not None else None, _stream_ptr(self.device)),
+                     "pdb_denoiser_grad_backward")
         return grads
 
     def camera_to_pose(self, R: torch.Tensor, T: torch.Tensor, focal: torch.Tensor, log_focal_length_bias=1.8, min_focal_length=0.1,

@@ -1,7 +1,8 @@
 // Training entry points of the denoiser: GaussianDiffusion.p_losses forward with every activation the backward needs saved in a
-// caller-owned workspace, the backward into 108 parameter gradients, camera_to_pose_encoding, and the host image of the dropout
-// masks.  Projections run through enqueue_tc_linear (TF32 products, fp32 accumulate) without its split-K regime, so every output
-// element is one CTA's fixed-order dot product; all other reductions are chunked fixed-order sums (csrc/train_common.cuh).
+// caller-owned workspace, the backward into 108 parameter gradients, the same pair for Denoiser.forward itself (eps from a given
+// x, backward from dL/deps into the parameters, x and z), camera_to_pose_encoding, and the host image of the dropout masks.
+// Projections run through enqueue_tc_linear (TF32 products, fp32 accumulate) without its split-K regime, so every output element
+// is one CTA's fixed-order dot product; all other reductions are chunked fixed-order sums (csrc/train_common.cuh).
 #include <cmath>
 #include <cstring>
 
@@ -12,7 +13,8 @@ using namespace pdb;
 
 namespace {
 
-constexpr int kMagic = 0x7d1a1e01;
+constexpr int kMagic = 0x7d1a1e01;          // workspace filled by pdb_train_forward (p_losses)
+constexpr int kMagicDenoiser = 0x7d1a1e02;  // workspace filled by pdb_denoiser_grad_forward (Denoiser.forward)
 
 // Workspace: a 64-float header, the saved activations, then the backward's scratch.  Offsets in floats, each 64-float aligned.
 struct TrainLayout {
@@ -106,26 +108,19 @@ DropCfg drop_cfg(uint32_t threshold, float scale, uint64_t seed) {
   return d;
 }
 
-}  // namespace
-
-extern "C" int64_t pdb_train_workspace_bytes(int32_t batch, int32_t frames) {
-  if (batch < 1 || frames < 1 || frames > kTrainMaxFrames) return 0;
-  return (int64_t)(TrainLayout(batch, frames).total * sizeof(float));
-}
-
-extern "C" int pdb_train_forward(pdb_context* c, const float* const* params, const float* x_start, const int32_t* t, const float* noise,
-                                 const float* z, int32_t batch, int32_t frames, float dropout_p, uint64_t seed, int32_t loss_type,
-                                 void* workspace, float* loss, float* x_t, float* x0, void* stream) {
-  if (!c) return PDB_ERR_INVALID;
-  Context* ctx = reinterpret_cast<Context*>(c);
-  if (int rc = check_params(ctx, params)) return rc;
-  if (!x_start || !t || !noise || !z || !workspace || !loss || !x_t || !x0) return ctx->fail(PDB_ERR_INVALID, "null argument");
+int check_forward_args(Context* ctx, int32_t batch, int32_t frames, float dropout_p, const void* workspace) {
   if (!aligned16(workspace)) return ctx->fail(PDB_ERR_INVALID, "workspace is not 16-byte aligned");
   if (batch < 1 || frames < 1) return ctx->fail(PDB_ERR_INVALID, "batch %d, frames %d", batch, frames);
   if (frames > kTrainMaxFrames) return ctx->fail(PDB_ERR_LIMIT, "training supports at most %d frames per sequence, got %d", kTrainMaxFrames, frames);
   if (!(dropout_p >= 0.f && dropout_p < 1.f)) return ctx->fail(PDB_ERR_INVALID, "dropout probability %g outside [0, 1)", (double)dropout_p);
-  if (loss_type != 0 && loss_type != 1) return ctx->fail(PDB_ERR_INVALID, "loss_type %d (0 = l1, 1 = l2)", loss_type);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  return PDB_OK;
+}
+
+// The forward both entry points share.  eps_mode (Denoiser.forward): the feed row is built from x_start = x, the tail writes eps
+// into `loss`, and noise, x_t, x0 and the saved diff are not used; the header then carries kMagicDenoiser.
+int enqueue_forward(Context* ctx, bool eps_mode, const float* const* params, const float* x_start, const int32_t* t, const float* noise,
+                    const float* z, int32_t batch, int32_t frames, float dropout_p, uint64_t seed, int32_t loss_type, void* workspace,
+                    float* loss, float* x_t, float* x0, cudaStream_t st) {
   PDB_CUDA(ctx, cudaSetDevice(ctx->device));
   if (int rc = set_attn_smem(ctx)) return rc;
   const TrainLayout L(batch, frames);
@@ -134,12 +129,16 @@ extern "C" int pdb_train_forward(pdb_context* c, const float* const* params, con
   const TrainSched sc = train_schedule();
   const DropCfg d = drop_cfg(dropout_threshold(dropout_p), 1.0f / (1.0f - dropout_p), seed);
   int* tsv = reinterpret_cast<int*>(ws + L.t);
-  TrainHeader hdr = {kMagic, batch, frames, loss_type, d.threshold, (uint32_t)seed, (uint32_t)(seed >> 32), d.scale, 0};
+  TrainHeader hdr = {eps_mode ? kMagicDenoiser : kMagic, batch, frames, loss_type, d.threshold, (uint32_t)seed, (uint32_t)(seed >> 32),
+                     d.scale, 0};
   train_launch(ctx, st, train_header_kernel, 1, 128, 0, hdr, reinterpret_cast<int*>(ws), t, tsv);
   auto W = [&](int i) { return params[i]; };
   // feed
   train_launch(ctx, st, train_time_mlp_kernel, B, 128, 0, tsv, W(0), W(1), W(2), W(3), ws + L.u1, ws + L.temb);
-  train_launch(ctx, st, train_feed_kernel, S, 256, 0, sc, x_start, noise, tsv, ws + L.temb, z, N, S, x_t, ws + L.feed);
+  if (eps_mode)
+    train_launch(ctx, st, train_feed_kernel<true>, S, 256, 0, sc, x_start, nullptr, tsv, ws + L.temb, z, N, S, nullptr, ws + L.feed);
+  else
+    train_launch(ctx, st, train_feed_kernel<false>, S, 256, 0, sc, x_start, noise, tsv, ws + L.temb, z, N, S, x_t, ws + L.feed);
   train_launch(ctx, st, train_copy_cols_kernel, blocks((long long)kDM * kFeedPad), 256, 0, W(4), kFirstIn, kDM, kFirstIn, ws + L.Wpad,
                kFeedPad);
   if (int rc = train_gemm(ctx, ws + L.feed, ws + L.Wpad, W(5), nullptr, ws + L.hin[0], S, kDM, kFeedPad, 0, st)) return rc;
@@ -162,10 +161,158 @@ extern "C" int pdb_train_forward(pdb_context* c, const float* const* params, con
   }
   const int tb = 6 + 12 * kLayers;
   if (int rc = train_gemm(ctx, ws + L.hin[kLayers], W(tb), W(tb + 1), nullptr, ws + L.u, S, kHid, kDM, 0, st)) return rc;
-  train_launch(ctx, st, train_tail_fwd_kernel, blocks(S, 8), 256, 0, sc, ws + L.u, W(tb + 2), W(tb + 3), W(tb + 4), W(tb + 5), tsv, x_t,
-               noise, N, S, loss_type, ws + L.stu, ws + L.r, ws + L.diff, loss, x0);
+  if (eps_mode)
+    train_launch(ctx, st, train_tail_fwd_kernel<true>, blocks(S, 8), 256, 0, sc, ws + L.u, W(tb + 2), W(tb + 3), W(tb + 4), W(tb + 5), tsv,
+                 nullptr, nullptr, N, S, 0, ws + L.stu, ws + L.r, nullptr, loss, nullptr);
+  else
+    train_launch(ctx, st, train_tail_fwd_kernel<false>, blocks(S, 8), 256, 0, sc, ws + L.u, W(tb + 2), W(tb + 3), W(tb + 4), W(tb + 5), tsv,
+                 x_t, noise, N, S, loss_type, ws + L.stu, ws + L.r, ws + L.diff, loss, x0);
   PDB_CUDA(ctx, cudaGetLastError());
   return PDB_OK;
+}
+
+// The backward both entry points share, from the workspace a forward with header magic `magic` filled.  grad_loss / grad_x0 seed the
+// tail as in p_losses; with magic == kMagicDenoiser grad_loss is dL/deps.  grads == NULL runs only the input-gradient chain (dropout,
+// linear-layer input gradients, LayerNorm and attention backward) towards grad_x / grad_z; each of those may be NULL.
+int enqueue_backward(Context* ctx, int magic, const float* const* params, void* workspace, const float* grad_loss, const float* grad_x0,
+                     float* const* grads, float* grad_x, float* grad_z, cudaStream_t st) {
+  PDB_CUDA(ctx, cudaSetDevice(ctx->device));
+  if (int rc = set_attn_smem(ctx)) return rc;
+  float* ws = static_cast<float*>(workspace);
+  TrainHeader hdr;
+  PDB_CUDA(ctx, cudaMemcpyAsync(&hdr, ws, sizeof(hdr), cudaMemcpyDeviceToHost, st));
+  PDB_CUDA(ctx, cudaStreamSynchronize(st));
+  if (hdr.magic != magic || hdr.batch < 1 || hdr.frames < 1 || hdr.frames > kTrainMaxFrames)
+    return ctx->fail(PDB_ERR_STATE, magic == kMagic ? "workspace does not hold a training forward"
+                                                    : "workspace does not hold a pdb_denoiser_grad_forward");
+  if (hdr.bad_t) return ctx->fail(PDB_ERR_INVALID, "the forward was given a timestep outside [0, %d)", kT);
+  const bool eps_mode = magic == kMagicDenoiser;
+  const TrainLayout L(hdr.batch, hdr.frames);
+  const int S = L.S, B = hdr.batch, N = hdr.frames;
+  const TrainSched sc = train_schedule();
+  const DropCfg d = drop_cfg(hdr.threshold, hdr.scale, (uint64_t)hdr.seed_lo | ((uint64_t)hdr.seed_hi << 32));
+  const int* tsv = reinterpret_cast<const int*>(ws + L.t);
+  auto W = [&](int i) { return params[i]; };
+  auto G = [&](int i) { return grads[i]; };
+  float *D0 = ws + L.D0, *D1 = ws + L.D1, *G1 = ws + L.G1, *G2 = ws + L.G2, *part = ws + L.part;
+  const LinearGrad lin = {ctx, S, L.Sp, ws + L.T1, ws + L.T2, ws + L.Wt, part, st};
+  const long long nd = (long long)S * kDM, nf = (long long)S * kFF;
+  // ---- tail ----
+  const int tb = 6 + 12 * kLayers;
+  float* dau = G2;  // [S, 128]
+  if (eps_mode)
+    train_launch(ctx, st, train_tail_bwd_kernel<true>, blocks(S, 8), 256, 0, sc, nullptr, grad_loss, nullptr, tsv, N, S, 0, W(tb + 4),
+                 ws + L.r, ws + L.deps, dau);
+  else
+    train_launch(ctx, st, train_tail_bwd_kernel<false>, blocks(S, 8), 256, 0, sc, ws + L.diff, grad_loss, grad_x0, tsv, N, S,
+                 hdr.loss_type, W(tb + 4), ws + L.r, ws + L.deps, dau);
+  if (grads) {
+    train_launch(ctx, st, train_w3_partial_kernel, kRedChunks, 128, 0, ws + L.deps, ws + L.r, S, part);
+    train_launch(ctx, st, train_chunk_sum_kernel, blocks(9 * 128), 256, 0, part, kRedChunks, 9 * 128, G(tb + 4));
+    lin.bias(ws + L.deps, S, 9, G(tb + 5));
+  }
+  float* du = G1;  // [S, 128]
+  train_launch(ctx, st, train_ln_bwd_kernel<kHid>, blocks(S, 8), 256, 0, dau, ws + L.u, ws + L.stu, W(tb + 2), nullptr, S, du,
+               G2 + (size_t)S * kHid);
+  if (grads) {
+    lin.bias(G2 + (size_t)S * kHid, S, kHid, G(tb + 2));
+    lin.bias(dau, S, kHid, G(tb + 3));
+    if (int rc = lin.weight(du, kHid, ws + L.hin[kLayers], kDM, G(tb))) return rc;
+    lin.bias(du, S, kHid, G(tb + 1));
+  }
+  if (int rc = lin.input(du, W(tb), kHid, kDM, D0)) return rc;
+  // ---- trunk, last layer first; D0 = gradient of the layer output ----
+  for (int l = kLayers - 1; l >= 0; --l) {
+    const int b = 6 + 12 * l;
+    float* dy2 = G1;
+    train_launch(ctx, st, train_dropout_kernel, blocks(nd), 256, 0, D0, nullptr, nullptr, dy2, nd, d, l, kSiteFF2);
+    if (int rc = lin.input(dy2, W(b + 6), kDM, kFF, G2)) return rc;  // d fd
+    if (grads) {
+      if (int rc = lin.weight(dy2, kDM, ws + L.fd[l], kFF, G(b + 6))) return rc;
+      lin.bias(dy2, S, kDM, G(b + 7));
+    }
+    train_launch(ctx, st, train_dropout_kernel, blocks(nf), 256, 0, G2, nullptr, ws + L.fd[l], G2, nf, d, l, kSiteRelu);  // d(FF1 output)
+    float* da2 = G1;
+    if (int rc = lin.input(G2, W(b + 4), kFF, kDM, da2)) return rc;
+    if (grads) {
+      if (int rc = lin.weight(G2, kFF, ws + L.a2[l], kDM, G(b + 4))) return rc;
+      lin.bias(G2, S, kFF, G(b + 5));
+    }
+    train_launch(ctx, st, train_ln_bwd_kernel<kDM>, blocks(S, 8), 256, 0, da2, ws + L.hmid[l], ws + L.st2[l], W(b + 10), D0, S, D1, G2);
+    if (grads) {
+      lin.bias(G2, S, kDM, G(b + 10));
+      lin.bias(da2, S, kDM, G(b + 11));
+    }
+    float* dy = G1;
+    train_launch(ctx, st, train_dropout_kernel, blocks(nd), 256, 0, D1, nullptr, nullptr, dy, nd, d, l, kSiteOut);
+    if (int rc = lin.input(dy, W(b + 2), kDM, kDM, G2)) return rc;  // d att
+    if (grads) {
+      if (int rc = lin.weight(dy, kDM, ws + L.att[l], kDM, G(b + 2))) return rc;
+      lin.bias(dy, S, kDM, G(b + 3));
+    }
+    float* dqkv = G1;
+    train_launch(ctx, st, train_attn_bwd_kernel, B * kHeads, 256, attn_bwd_smem(N), ws + L.qkv[l], ws + L.P[l], G2, N, d, l, dqkv);
+    float* da1 = G2;
+    if (int rc = lin.input(dqkv, W(b + 0), 3 * kDM, kDM, da1)) return rc;
+    if (grads) {
+      if (int rc = lin.weight(dqkv, 3 * kDM, ws + L.a1[l], kDM, G(b + 0))) return rc;
+      lin.bias(dqkv, S, 3 * kDM, G(b + 1));
+    }
+    train_launch(ctx, st, train_ln_bwd_kernel<kDM>, blocks(S, 8), 256, 0, da1, ws + L.hin[l], ws + L.st1[l], W(b + 8), D1, S, D0, G1);
+    if (grads) {
+      lin.bias(G1, S, kDM, G(b + 8));
+      lin.bias(da1, S, kDM, G(b + 9));
+    }
+  }
+  // ---- _first and the time MLP ----
+  if (grads) {
+    if (int rc = lin.weight(D0, kDM, ws + L.feed, kFeedPad, ws + L.dWf)) return rc;
+    train_launch(ctx, st, train_copy_cols_kernel, blocks((long long)kDM * kFirstIn), 256, 0, ws + L.dWf, kFeedPad, kDM, kFirstIn, G(4),
+                 kFirstIn);
+    lin.bias(D0, S, kDM, G(5));
+    train_launch(ctx, st, train_dtemb_kernel, B, 256, 0, D0, N, W(4), ws + L.dtemb);
+    train_launch(ctx, st, train_time_du_kernel, blocks((long long)B * 128), 256, 0, ws + L.dtemb, ws + L.u1, W(2), B, ws + L.du1);
+    train_launch(ctx, st, train_time_dw_kernel, blocks(128 * 128), 256, 0, ws + L.dtemb, ws + L.u1, tsv, B, 128, 1, G(2), G(3));
+    train_launch(ctx, st, train_time_dw_kernel, blocks(128 * 256), 256, 0, ws + L.du1, ws + L.u1, tsv, B, 256, 0, G(0), G(1));
+  }
+  if (grad_z) {
+    // dz = dh0 . W_first[:, 317:701]: the column block starts at float 317, which TMA cannot address, so it is copied to an
+    // aligned [512, 384] buffer (the _first weight-gradient staging area, free by now) and then read K-major like every dX
+    float* Wz = ws + L.dWf;
+    train_launch(ctx, st, train_copy_cols_kernel, blocks((long long)kDM * kZ), 256, 0, W(4) + 317, kFirstIn, kDM, kZ, Wz, kZ);
+    if (int rc = lin.input(D0, Wz, kDM, kZ, grad_z)) return rc;
+  }
+  if (grad_x) {
+    // dfeed[:, 0:189] = dh0 . W_first[:, 0:189] through the same staging area (zero-padded to 192 columns, the GEMM's 64-multiple),
+    // into G1 (free after the trunk); then the harmonic embedding's chain rule per element
+    constexpr int kXCols = 189, kXPad = 192;
+    float* Wx = ws + L.dWf;
+    train_launch(ctx, st, train_copy_cols_kernel, blocks((long long)kDM * kXPad), 256, 0, W(4), kFirstIn, kDM, kXCols, Wx, kXPad);
+    if (int rc = lin.input(D0, Wx, kDM, kXPad, G1)) return rc;
+    train_launch(ctx, st, train_dx_kernel, blocks((long long)S * 9), 256, 0, ws + L.feed, G1, S, grad_x);
+  }
+  PDB_CUDA(ctx, cudaGetLastError());
+  return PDB_OK;
+}
+
+}  // namespace
+
+extern "C" int64_t pdb_train_workspace_bytes(int32_t batch, int32_t frames) {
+  if (batch < 1 || frames < 1 || frames > kTrainMaxFrames) return 0;
+  return (int64_t)(TrainLayout(batch, frames).total * sizeof(float));
+}
+
+extern "C" int pdb_train_forward(pdb_context* c, const float* const* params, const float* x_start, const int32_t* t, const float* noise,
+                                 const float* z, int32_t batch, int32_t frames, float dropout_p, uint64_t seed, int32_t loss_type,
+                                 void* workspace, float* loss, float* x_t, float* x0, void* stream) {
+  if (!c) return PDB_ERR_INVALID;
+  Context* ctx = reinterpret_cast<Context*>(c);
+  if (int rc = check_params(ctx, params)) return rc;
+  if (!x_start || !t || !noise || !z || !workspace || !loss || !x_t || !x0) return ctx->fail(PDB_ERR_INVALID, "null argument");
+  if (int rc = check_forward_args(ctx, batch, frames, dropout_p, workspace)) return rc;
+  if (loss_type != 0 && loss_type != 1) return ctx->fail(PDB_ERR_INVALID, "loss_type %d (0 = l1, 1 = l2)", loss_type);
+  return enqueue_forward(ctx, false, params, x_start, t, noise, z, batch, frames, dropout_p, seed, loss_type, workspace, loss, x_t, x0,
+                         static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int pdb_train_backward(pdb_context* c, const float* const* params, void* workspace, const float* grad_loss, const float* grad_x0,
@@ -182,91 +329,35 @@ extern "C" int pdb_train_backward_z(pdb_context* c, const float* const* params, 
   if (grad_z && !aligned16(grad_z)) return ctx->fail(PDB_ERR_INVALID, "grad_z is not 16-byte aligned");
   for (int i = 0; i < PDB_NUM_WEIGHT_TENSORS; ++i)
     if (!grads[i] || !aligned16(grads[i])) return ctx->fail(PDB_ERR_INVALID, "gradient %d is null or not 16-byte aligned", i);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  PDB_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (int rc = set_attn_smem(ctx)) return rc;
-  float* ws = static_cast<float*>(workspace);
-  TrainHeader hdr;
-  PDB_CUDA(ctx, cudaMemcpyAsync(&hdr, ws, sizeof(hdr), cudaMemcpyDeviceToHost, st));
-  PDB_CUDA(ctx, cudaStreamSynchronize(st));
-  if (hdr.magic != kMagic || hdr.batch < 1 || hdr.frames < 1 || hdr.frames > kTrainMaxFrames)
-    return ctx->fail(PDB_ERR_STATE, "workspace does not hold a training forward");
-  if (hdr.bad_t) return ctx->fail(PDB_ERR_INVALID, "the forward was given a timestep outside [0, %d)", kT);
-  const TrainLayout L(hdr.batch, hdr.frames);
-  const int S = L.S, B = hdr.batch, N = hdr.frames;
-  const TrainSched sc = train_schedule();
-  const DropCfg d = drop_cfg(hdr.threshold, hdr.scale, (uint64_t)hdr.seed_lo | ((uint64_t)hdr.seed_hi << 32));
-  const int* tsv = reinterpret_cast<const int*>(ws + L.t);
-  auto W = [&](int i) { return params[i]; };
-  auto G = [&](int i) { return grads[i]; };
-  float *D0 = ws + L.D0, *D1 = ws + L.D1, *G1 = ws + L.G1, *G2 = ws + L.G2, *part = ws + L.part;
-  const LinearGrad lin = {ctx, S, L.Sp, ws + L.T1, ws + L.T2, ws + L.Wt, part, st};
-  const long long nd = (long long)S * kDM, nf = (long long)S * kFF;
-  // ---- tail ----
-  const int tb = 6 + 12 * kLayers;
-  float* dau = G2;  // [S, 128]
-  train_launch(ctx, st, train_tail_bwd_kernel, blocks(S, 8), 256, 0, sc, ws + L.diff, grad_loss, grad_x0, tsv, N, S, hdr.loss_type,
-               W(tb + 4), ws + L.r, ws + L.deps, dau);
-  train_launch(ctx, st, train_w3_partial_kernel, kRedChunks, 128, 0, ws + L.deps, ws + L.r, S, part);
-  train_launch(ctx, st, train_chunk_sum_kernel, blocks(9 * 128), 256, 0, part, kRedChunks, 9 * 128, G(tb + 4));
-  lin.bias(ws + L.deps, S, 9, G(tb + 5));
-  float* du = G1;  // [S, 128]
-  train_launch(ctx, st, train_ln_bwd_kernel<kHid>, blocks(S, 8), 256, 0, dau, ws + L.u, ws + L.stu, W(tb + 2), nullptr, S, du,
-               G2 + (size_t)S * kHid);
-  lin.bias(G2 + (size_t)S * kHid, S, kHid, G(tb + 2));
-  lin.bias(dau, S, kHid, G(tb + 3));
-  if (int rc = lin.weight(du, kHid, ws + L.hin[kLayers], kDM, G(tb))) return rc;
-  lin.bias(du, S, kHid, G(tb + 1));
-  if (int rc = lin.input(du, W(tb), kHid, kDM, D0)) return rc;
-  // ---- trunk, last layer first; D0 = gradient of the layer output ----
-  for (int l = kLayers - 1; l >= 0; --l) {
-    const int b = 6 + 12 * l;
-    float* dy2 = G1;
-    train_launch(ctx, st, train_dropout_kernel, blocks(nd), 256, 0, D0, nullptr, nullptr, dy2, nd, d, l, kSiteFF2);
-    if (int rc = lin.input(dy2, W(b + 6), kDM, kFF, G2)) return rc;  // d fd
-    if (int rc = lin.weight(dy2, kDM, ws + L.fd[l], kFF, G(b + 6))) return rc;
-    lin.bias(dy2, S, kDM, G(b + 7));
-    train_launch(ctx, st, train_dropout_kernel, blocks(nf), 256, 0, G2, nullptr, ws + L.fd[l], G2, nf, d, l, kSiteRelu);  // d(FF1 output)
-    float* da2 = G1;
-    if (int rc = lin.input(G2, W(b + 4), kFF, kDM, da2)) return rc;
-    if (int rc = lin.weight(G2, kFF, ws + L.a2[l], kDM, G(b + 4))) return rc;
-    lin.bias(G2, S, kFF, G(b + 5));
-    train_launch(ctx, st, train_ln_bwd_kernel<kDM>, blocks(S, 8), 256, 0, da2, ws + L.hmid[l], ws + L.st2[l], W(b + 10), D0, S, D1, G2);
-    lin.bias(G2, S, kDM, G(b + 10));
-    lin.bias(da2, S, kDM, G(b + 11));
-    float* dy = G1;
-    train_launch(ctx, st, train_dropout_kernel, blocks(nd), 256, 0, D1, nullptr, nullptr, dy, nd, d, l, kSiteOut);
-    if (int rc = lin.input(dy, W(b + 2), kDM, kDM, G2)) return rc;  // d att
-    if (int rc = lin.weight(dy, kDM, ws + L.att[l], kDM, G(b + 2))) return rc;
-    lin.bias(dy, S, kDM, G(b + 3));
-    float* dqkv = G1;
-    train_launch(ctx, st, train_attn_bwd_kernel, B * kHeads, 256, attn_bwd_smem(N), ws + L.qkv[l], ws + L.P[l], G2, N, d, l, dqkv);
-    float* da1 = G2;
-    if (int rc = lin.input(dqkv, W(b + 0), 3 * kDM, kDM, da1)) return rc;
-    if (int rc = lin.weight(dqkv, 3 * kDM, ws + L.a1[l], kDM, G(b + 0))) return rc;
-    lin.bias(dqkv, S, 3 * kDM, G(b + 1));
-    train_launch(ctx, st, train_ln_bwd_kernel<kDM>, blocks(S, 8), 256, 0, da1, ws + L.hin[l], ws + L.st1[l], W(b + 8), D1, S, D0, G1);
-    lin.bias(G1, S, kDM, G(b + 8));
-    lin.bias(da1, S, kDM, G(b + 9));
-  }
-  // ---- _first and the time MLP ----
-  if (int rc = lin.weight(D0, kDM, ws + L.feed, kFeedPad, ws + L.dWf)) return rc;
-  train_launch(ctx, st, train_copy_cols_kernel, blocks((long long)kDM * kFirstIn), 256, 0, ws + L.dWf, kFeedPad, kDM, kFirstIn, G(4),
-               kFirstIn);
-  lin.bias(D0, S, kDM, G(5));
-  train_launch(ctx, st, train_dtemb_kernel, B, 256, 0, D0, N, W(4), ws + L.dtemb);
-  train_launch(ctx, st, train_time_du_kernel, blocks((long long)B * 128), 256, 0, ws + L.dtemb, ws + L.u1, W(2), B, ws + L.du1);
-  train_launch(ctx, st, train_time_dw_kernel, blocks(128 * 128), 256, 0, ws + L.dtemb, ws + L.u1, tsv, B, 128, 1, G(2), G(3));
-  train_launch(ctx, st, train_time_dw_kernel, blocks(128 * 256), 256, 0, ws + L.du1, ws + L.u1, tsv, B, 256, 0, G(0), G(1));
-  if (grad_z) {
-    // dz = dh0 . W_first[:, 317:701]: the column block starts at float 317, which TMA cannot address, so it is copied to an
-    // aligned [512, 384] buffer (the _first weight-gradient staging area, free by now) and then read K-major like every dX
-    float* Wz = ws + L.dWf;
-    train_launch(ctx, st, train_copy_cols_kernel, blocks((long long)kDM * kZ), 256, 0, W(4) + 317, kFirstIn, kDM, kZ, Wz, kZ);
-    if (int rc = lin.input(D0, Wz, kDM, kZ, grad_z)) return rc;
-  }
-  PDB_CUDA(ctx, cudaGetLastError());
-  return PDB_OK;
+  return enqueue_backward(ctx, kMagic, params, workspace, grad_loss, grad_x0, grads, nullptr, grad_z, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int pdb_denoiser_grad_forward(pdb_context* c, const float* const* params, const float* x, const int32_t* t, const float* z,
+                                         int32_t batch, int32_t frames, float dropout_p, uint64_t seed, void* workspace, float* eps,
+                                         void* stream) {
+  if (!c) return PDB_ERR_INVALID;
+  Context* ctx = reinterpret_cast<Context*>(c);
+  if (int rc = check_params(ctx, params)) return rc;
+  if (!x || !t || !z || !workspace || !eps) return ctx->fail(PDB_ERR_INVALID, "null argument");
+  if (int rc = check_forward_args(ctx, batch, frames, dropout_p, workspace)) return rc;
+  return enqueue_forward(ctx, true, params, x, t, nullptr, z, batch, frames, dropout_p, seed, 0, workspace, eps, nullptr, nullptr,
+                         static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int pdb_denoiser_grad_backward(pdb_context* c, const float* const* params, void* workspace, const float* grad_eps,
+                                          float* const* grads, float* grad_x, float* grad_z, void* stream) {
+  if (!c) return PDB_ERR_INVALID;
+  Context* ctx = reinterpret_cast<Context*>(c);
+  if (int rc = check_params(ctx, params)) return rc;
+  if (!workspace || !grad_eps) return ctx->fail(PDB_ERR_INVALID, "null argument");
+  if (!grads && !grad_x && !grad_z) return ctx->fail(PDB_ERR_INVALID, "no gradient requested");
+  if ((grad_x && !aligned16(grad_x)) || (grad_z && !aligned16(grad_z)))
+    return ctx->fail(PDB_ERR_INVALID, "grad_x or grad_z is not 16-byte aligned");
+  if (grads)
+    for (int i = 0; i < PDB_NUM_WEIGHT_TENSORS; ++i)
+      if (!grads[i] || !aligned16(grads[i])) return ctx->fail(PDB_ERR_INVALID, "gradient %d is null or not 16-byte aligned", i);
+  return enqueue_backward(ctx, kMagicDenoiser, params, workspace, grad_eps, nullptr, grads, grad_x, grad_z,
+                          static_cast<cudaStream_t>(stream));
 }
 
 // camera_to_pose_encoding, "absT_quaR_logFL" (util/camera_transform.py:108-129) with pytorch3d's matrix_to_quaternion followed by

@@ -86,7 +86,9 @@ __global__ void train_time_mlp_kernel(const int* __restrict__ t, const float* __
 }
 
 // q_sample + feed row: x_t = sqrt(abar_t) x_start + sqrt(1 - abar_t) noise (products rounded separately, as torch evaluates them);
-// feed = [sin(x_t 2^k) | cos(x_t 2^k) | x_t | t-embedding | z | pivot one-hot | 0 0]
+// feed = [sin(x_t 2^k) | cos(x_t 2^k) | x_t | t-embedding | z | pivot one-hot | 0 0].
+// kFromX (Denoiser.forward): the row is built from the given x_start = x itself; noise and x_t are not read or written.
+template <bool kFromX>
 __global__ void train_feed_kernel(const __grid_constant__ TrainSched sc, const float* __restrict__ x_start, const float* __restrict__ noise,
                                   const int* __restrict__ t, const float* __restrict__ temb, const float* __restrict__ z, int frames,
                                   int S, float* __restrict__ x_t, float* __restrict__ feed) {
@@ -95,9 +97,13 @@ __global__ void train_feed_kernel(const __grid_constant__ TrainSched sc, const f
   const int b = s / frames, n = s - b * frames, tb = t[b];
   __shared__ float xs[9];
   if (threadIdx.x < 9) {
-    const float v = __fadd_rn(__fmul_rn(sc.c[tb][0], x_start[s * 9 + threadIdx.x]), __fmul_rn(sc.c[tb][1], noise[s * 9 + threadIdx.x]));
-    xs[threadIdx.x] = v;
-    x_t[s * 9 + threadIdx.x] = v;
+    if (kFromX) {
+      xs[threadIdx.x] = x_start[s * 9 + threadIdx.x];
+    } else {
+      const float v = __fadd_rn(__fmul_rn(sc.c[tb][0], x_start[s * 9 + threadIdx.x]), __fmul_rn(sc.c[tb][1], noise[s * 9 + threadIdx.x]));
+      xs[threadIdx.x] = v;
+      x_t[s * 9 + threadIdx.x] = v;
+    }
   }
   __syncthreads();
   float* row = feed + (size_t)s * kFeedPad;
@@ -199,6 +205,8 @@ __global__ void __launch_bounds__(256) train_attn_fwd_kernel(const float* __rest
 }
 
 // tail: LayerNorm(128) -> ReLU -> Linear(128, 9) -> eps; x_0_pred and the element-wise loss (reduction "none").  Warp per token.
+// kEps (Denoiser.forward): eps itself is written to `loss`; x_t, noise, diff and x0 are not touched.
+template <bool kEps>
 __global__ void train_tail_fwd_kernel(const __grid_constant__ TrainSched sc, const float* __restrict__ u, const float* __restrict__ g,
                                       const float* __restrict__ bta, const float* __restrict__ w3, const float* __restrict__ b3,
                                       const int* __restrict__ t, const float* __restrict__ x_t, const float* __restrict__ noise, int frames,
@@ -226,7 +234,9 @@ __global__ void train_tail_fwd_kernel(const __grid_constant__ TrainSched sc, con
 #pragma unroll
     for (int i = 0; i < 4; ++i) a = fmaf(w3[o * 128 + lane + 32 * i], v[i], a);
     const float eps = warp_sum(a) + b3[o];
-    if (lane == 0) {
+    if (kEps) {
+      if (lane == 0) loss[s * 9 + o] = eps;
+    } else if (lane == 0) {
       const int e = s * 9 + o;
       x0[e] = __fsub_rn(__fmul_rn(sc.c[tb][2], x_t[e]), __fmul_rn(sc.c[tb][3], eps));
       const float dd = eps - noise[e];
@@ -238,7 +248,8 @@ __global__ void train_tail_fwd_kernel(const __grid_constant__ TrainSched sc, con
 
 // ---- backward ----------------------------------------------------------------------------------------------------------------
 // tail backward, one warp per token: deps = grad_loss * dloss/deps - sqrt_recipm1(t) * grad_x0 (stored [S,9] for the _last.3
-// gradients); dr = deps W3; d(LN out) = dr * (r > 0)
+// gradients); dr = deps W3; d(LN out) = dr * (r > 0).  kEps (Denoiser.forward's backward): deps = grad_loss = dL/deps.
+template <bool kEps>
 __global__ void train_tail_bwd_kernel(const __grid_constant__ TrainSched sc, const float* __restrict__ diff, const float* __restrict__ gl,
                                       const float* __restrict__ gx0, const int* __restrict__ t, int frames, int S, int l2,
                                       const float* __restrict__ w3, const float* __restrict__ r, float* __restrict__ deps,
@@ -250,6 +261,10 @@ __global__ void train_tail_bwd_kernel(const __grid_constant__ TrainSched sc, con
 #pragma unroll
   for (int o = 0; o < 9; ++o) {
     const int e = s * 9 + o;
+    if (kEps) {
+      de[o] = gl[e];
+      continue;
+    }
     const float dd = diff[e];
     const float dl = l2 ? 2.0f * dd : (float)((dd > 0.f) - (dd < 0.f));
     float v = gl ? gl[e] * dl : 0.f;
@@ -399,6 +414,24 @@ __global__ void train_time_dw_kernel(const float* __restrict__ dy, const float* 
   }
   dw[i] = a;
   if (k == 0) db[o] = bsum;
+}
+
+// dL/dx of the harmonic feed columns (Denoiser.forward's backward), thread per (token, pose dimension i):
+// dx[i] = dfeed[180 + i] + sum_k 2^k (cos(2^k x_i) dfeed[10 i + k] - sin(2^k x_i) dfeed[90 + 10 i + k]), with sin and cos read back
+// from the saved feed row; dfeed [S, 192] holds dL/dfeed of columns 0..188
+__global__ void train_dx_kernel(const float* __restrict__ feed, const float* __restrict__ dfeed, int S, float* __restrict__ dx) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= S * 9) return;
+  const int s = e / 9, i = e - s * 9;
+  const float* f = feed + (size_t)s * kFeedPad;
+  const float* g = dfeed + (size_t)s * 192;
+  float a = 0.f;
+#pragma unroll
+  for (int k = 0; k < 10; ++k) {
+    const int c = 10 * i + k;
+    a = fmaf((float)(1 << k), fmaf(f[90 + c], g[c], -f[c] * g[90 + c]), a);
+  }
+  dx[e] = g[180 + i] + a;
 }
 
 }  // namespace

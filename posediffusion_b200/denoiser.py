@@ -11,6 +11,7 @@ from typing import Dict, List
 
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 from . import _native
 from .synthetic import denoiser_param_shapes
@@ -79,6 +80,36 @@ class _DiffusionLoss(torch.autograd.Function):
         return (None, None, None, None, None, grad_z, *grads)
 
 
+class _DenoiserEps(torch.autograd.Function):
+    """Native Denoiser.forward with a backward: the forward (pdb_denoiser_grad_forward) saves its activations in a workspace tensor
+    that this graph node owns; the backward (pdb_denoiser_grad_backward) returns dL/dx, dL/dz and the 108 parameter gradients, each
+    only when asked for.  Without a parameter that needs a gradient the weight-gradient kernels are skipped altogether.  The
+    parameters are saved for backward, so changing one in place between the two raises torch's version error."""
+
+    @staticmethod
+    def forward(fctx, ctx, t, dropout_p, seed, x, z, *params):
+        ws, eps = ctx.denoiser_grad_forward(params, x, t, z, dropout_p, seed)
+        fctx.native, fctx.ws = ctx, ws
+        fctx.save_for_backward(*params)
+        return eps
+
+    @staticmethod
+    @once_differentiable
+    def backward(fctx, grad_eps):
+        params = fctx.saved_tensors
+        if fctx.ws is None:
+            raise RuntimeError("the native denoiser graph was already backpropagated and its workspace released "
+                               "(a second backward through one Denoiser.forward is not supported)")
+        need = fctx.needs_input_grad
+        grad_x = torch.empty(grad_eps.shape, device=params[0].device, dtype=torch.float32) if need[4] else None
+        grad_z = torch.empty(grad_eps.shape[:2] + (_native.Z_DIM,), device=params[0].device, dtype=torch.float32) if need[5] else None
+        want_params = any(need[6:])
+        grads = fctx.native.denoiser_grad_backward(params, fctx.ws, grad_eps.float().contiguous(), want_params, grad_x, grad_z)
+        fctx.ws = None
+        pgrads = [g if n else None for g, n in zip(grads, need[6:])] if want_params else [None] * len(params)
+        return (None, None, None, None, grad_x, grad_z, *pgrads)
+
+
 class Denoiser(nn.Module):
     def __init__(self, TRANSFORMER: Dict, target_dim: int = 9, pivot_cam_onehot: bool = True, z_dim: int = 384,
                  mlp_hidden_dim: int = 128):
@@ -108,6 +139,7 @@ class Denoiser(nn.Module):
         self.dropout_p = float(_cfg_get(TRANSFORMER, "dropout", 0.1))  # applied by the training kernels in train() mode only
         self._native_token = _native.module_token()  # identity for the context's weight cache (never reused, unlike id())
         self._native_epoch = 0
+        self.autograd_enabled = False  # enable_autograd(); a plain attribute, so not part of state_dict
 
     # ---- native weight sync -------------------------------------------------------------------------
     def ordered_parameters(self) -> List[torch.Tensor]:
@@ -154,8 +186,49 @@ class Denoiser(nn.Module):
         args = (x_start.detach().contiguous().float(), t.to(torch.int32).contiguous(), noise.detach().contiguous().float())
         return _DiffusionLoss.apply(ctx, args, float(dropout_p), seed_v, loss_type, z.contiguous().float(), *params)
 
+    def enable_autograd(self, enabled: bool = True) -> "Denoiser":
+        """Opt in (or back out) of the differentiable forward: while enabled, every `forward` call runs on the training engine
+        (TF32 projections, fp32 elsewhere) with one timestep per sequence, dropout in train() mode, and a backward into the
+        parameters, x and z.  While disabled (the default) `forward` is the exact-fp32 inference kernel with one timestep per
+        batch and a detached output.  The sampler entry points never read this flag.  Returns the module."""
+        self.autograd_enabled = bool(enabled)
+        return self
+
+    def _forward_autograd(self, x: torch.Tensor, t, z: torch.Tensor) -> torch.Tensor:
+        params = self.ordered_parameters()
+        device = params[0].device
+        if device.type != "cuda":
+            raise _native.NativeError("Denoiser parameters are on the CPU: call .to('cuda') (no CPU fallback)")
+        for name, v in (("x", x), ("z", z)):
+            if not v.is_cuda:
+                raise _native.NativeError(f"{name} must be a CUDA tensor (posediffusion_b200 has no CPU fallback)")
+        B = x.shape[0]
+        t = torch.as_tensor(t)
+        if t.is_floating_point() or t.is_complex() or t.dtype == torch.bool:
+            raise TypeError(f"t must be an integer tensor, got {t.dtype}")
+        if t.dim() > 1 or t.numel() not in (1, B):
+            raise ValueError(f"t must have shape [{B}], [1] or [], got {tuple(t.shape)}")
+        p = self.dropout_p if self.training else 0.0
+        # t out of range and the dropout seed (drawn on the device generator when dropout is active) in one device-to-host read
+        bad = ((t < 0) | (t >= _native.NUM_TIMESTEPS)).any().view(1).to(device, torch.int64)
+        if p > 0:
+            seed, bad_v = torch.cat([torch.randint(0, 2**63 - 1, (1,), device=device), bad]).tolist()
+        else:
+            seed, bad_v = 0, int(bad.item())
+        if bad_v:
+            raise IndexError(f"timesteps must lie in [0, {_native.NUM_TIMESTEPS})")
+        t32 = t.reshape(-1).to(device, torch.int32).expand(B).contiguous()
+        ctx = _native.Context.get(device)
+        xf, zf = x.float().contiguous(), z.float().contiguous()
+        if not (torch.is_grad_enabled() and (xf.requires_grad or zf.requires_grad or any(q.requires_grad for q in params))):
+            return ctx.denoiser_grad_forward(params, xf.detach(), t32, zf.detach(), p, seed)[1]  # the workspace is released here
+        return _DenoiserEps.apply(ctx, t32, p, seed, xf, zf, *params)
+
     def forward(self, x: torch.Tensor, t: torch.Tensor, z: torch.Tensor) -> torch.Tensor:
-        """x [B,N,9], t [B] (all entries equal, as the sampler passes them), z [B,N,384] -> eps [B,N,9]."""
+        """x [B,N,9], t [B] (all entries equal, as the sampler passes them), z [B,N,384] -> eps [B,N,9].
+        After enable_autograd(): t [B] (or one value for all) may differ per sequence and eps is differentiable."""
+        if self.autograd_enabled:
+            return self._forward_autograd(x, t, z)
         ctx = self.native_context()
         t_host = t.reshape(-1)
         step = int(t_host[0]) if t_host.numel() else 0
