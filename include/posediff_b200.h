@@ -113,6 +113,15 @@ int pdb_debug_tc_swap(pdb_context* ctx, int32_t on);
  * the 80 KB flagged tiles loads L2).  Debug / measurement switch (environment: PDB_DEN_FLAG). */
 int pdb_debug_denoiser_handover(pdb_context* ctx, int32_t flagged);
 
+/* Reproducible mode.  on = 1: every sampling entry (pdb_ggs, pdb_sample_loop*, pdb_p_sample, pdb_denoiser_forward) returns the
+ * same bits on every call with the same inputs (weights, z, draws, match sets, GGS config) on the same library build and GPU
+ * model, whatever else runs on the GPU: GGS runs a kernel whose floating-point sums all have a fixed order and exchanges its
+ * partial gradients through the flag-carrying slots (no one-hop reductions), and the tensor-core GEMMs run without split-K.
+ * on = 0 (the default): the faster kernels, whose floating-point sums depend on scheduling.  Affects only work enqueued after the
+ * call; the debug outputs (pdb_debug_ggs_clocks, pdb_sampson_eval) are outside the contract.  Any other value: PDB_ERR_INVALID,
+ * the mode unchanged. */
+int pdb_set_reproducible(pdb_context* ctx, int on);
+
 /* Denoiser engine: 0 = auto (exact-fp32 persistent kernel below 128 tokens per GPU, wgmma/TMA tensor-core tiles with TF32
  * products at or above), 1 = always fp32, 2 = always tensor cores. */
 int pdb_denoiser_engine(pdb_context* ctx, int32_t mode);

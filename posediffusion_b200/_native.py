@@ -70,6 +70,7 @@ EXPORTS = {
     "pdb_profile_read": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int64), C.POINTER(C.c_double), C.POINTER(C.c_int64)]),
     "pdb_debug_ggs_clocks": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32]),
     "pdb_denoiser_engine": (C.c_int, [C.c_void_p, C.c_int32]),
+    "pdb_set_reproducible": (C.c_int, [C.c_void_p, C.c_int]),
     "pdb_debug_tc_linear": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     "pdb_schedule_table": (C.c_int, [C.c_void_p, C.c_double, C.c_double]),
     "pdb_ddim_table": (C.c_int, [C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_void_p, C.c_void_p]),
@@ -345,6 +346,7 @@ class Context:
         self.handle = handle
         self.weights_key = None
         self.ggs_layout = {v: k for k, v in GGS_LAYOUTS.items()}[int(self.lib.pdb_ggs_layout_get(handle))]
+        self.reproducible = False  # the library's mode (pdb_set_reproducible), kept in step with torch's switch by _sync_reproducible
 
     @classmethod
     def get(cls, device) -> "Context":
@@ -359,6 +361,14 @@ class Context:
     def _ok(self, rc: int, what: str):
         if rc != 0:
             raise NativeError(f"{what} failed ({rc}): {self.lib.pdb_last_error(self.handle).decode()}")
+
+    def _sync_reproducible(self):
+        """Mirror torch.use_deterministic_algorithms into the library before a sampling call is enqueued: while it is on, every
+        sampling entry gives the same bits on every call (pdb_set_reproducible).  The setter runs only when the switch changed."""
+        on = torch.are_deterministic_algorithms_enabled()
+        if on != self.reproducible:
+            self._ok(self.lib.pdb_set_reproducible(self.handle, int(on)), "pdb_set_reproducible")
+            self.reproducible = on
 
     @property
     def launch_count(self) -> int:
@@ -681,6 +691,7 @@ class Context:
         B, N, _ = x.shape
         _check_dev(x, "x", self.device, (B, N, TARGET_DIM))
         _check_dev(z, "z", self.device, (B, N, Z_DIM))
+        self._sync_reproducible()
         eps = torch.empty_like(x)
         self._ok(self.lib.pdb_denoiser_forward(self.handle, x.data_ptr(), int(t), z.data_ptr(), B, N, eps.data_ptr(),
                                                _stream_ptr(self.device)), "pdb_denoiser_forward")
@@ -692,6 +703,7 @@ class Context:
         _check_dev(z, "z", self.device, (B, N, Z_DIM))
         if noise is not None:
             _check_dev(noise, "noise", self.device, (B, N, TARGET_DIM))
+        self._sync_reproducible()
         pred, mean, x0 = torch.empty_like(x), torch.empty_like(x), torch.empty_like(x)
         self._ok(self.lib.pdb_p_sample(self.handle, x.data_ptr(), int(t), z.data_ptr(),
                                        noise.data_ptr() if noise is not None else None, B, N, pred.data_ptr(),
@@ -745,6 +757,7 @@ class Context:
         B = len(problems)
         _check_dev(pose, "model_mean", self.device, (B, problems[0].frames, TARGET_DIM))
         stats = torch.zeros(B * GGS_STATS_DTYPE.itemsize, dtype=torch.uint8, device=self.device) if want_stats else None
+        self._sync_reproducible()
         conf = ggs_config_struct(cfg)
         self._ok(self.lib.pdb_ggs(self.handle, self._problem_array(problems), B, pose.data_ptr(), C.byref(conf),
                                   stats.data_ptr() if want_stats else None, _stream_ptr(self.device)), "pdb_ggs")
@@ -764,6 +777,7 @@ class Context:
         stats = None
         if want_stats and problems and stats_rows:
             stats = torch.zeros(stats_rows * B * GGS_STATS_DTYPE.itemsize, dtype=torch.uint8, device=self.device)
+        self._sync_reproducible()
         conf = ggs_config_struct(cfg) if problems else None
         self._ok(getattr(self.lib, entry)(self.handle, z.data_ptr(), draws.data_ptr(), B, N, *ddim_args,
                                           self._problem_array(problems) if problems else None, len(problems) if problems else 0,
@@ -811,6 +825,7 @@ class Context:
         self._check_host_buffers(z, draws, NUM_TIMESTEPS + 1, trail_out, NUM_TIMESTEPS + 1, stats_out, guided)
         if problems:
             self._check_problems(problems, B, N)
+        self._sync_reproducible()
         conf = ggs_config_struct(cfg) if problems else None
         with torch.cuda.device(self.device):
             self._ok(self.lib.pdb_sample_loop_host(self.handle, z.ctypes.data, draws.ctypes.data, B, N,
@@ -827,6 +842,7 @@ class Context:
         B, N, _ = z.shape
         self._check_host_buffers(z, draws, draw_slots, trail_out, trail_slots, stats_out, stats_rows)
         ptrs, counts, shape, _keep = self._host_match_arrays(matches_dicts, B, N)
+        self._sync_reproducible()
         conf = ggs_config_struct(cfg)
         with torch.cuda.device(self.device):
             rc = getattr(self.lib, entry)(self.handle, z.ctypes.data, draws.ctypes.data, B, N, *ddim_args, ptrs[0], ptrs[1], ptrs[2],

@@ -23,6 +23,9 @@ struct GgsBatch {
 template <bool kEval, bool kPaired, bool kProbe = false, bool kLean = false>
 __global__ void __launch_bounds__(kGgsThreads, 1)
 ggs_entry(const __grid_constant__ GgsBatch batch, const __grid_constant__ GgsParams P);
+template <bool kPaired>
+__global__ void __launch_bounds__(kGgsThreads, 1)
+ggs_entry_repro(const __grid_constant__ GgsBatch batch, const __grid_constant__ GgsParams P);
 
 // Exchange workspace of one sequence: double-buffered slots of its CTAs (xch1) and of its group leaders (xch2).
 size_t ggs_ws_slots_bytes(int frames, int cpp, int group) {
@@ -113,6 +116,14 @@ int pdb_device_info(const pdb_context* c, int32_t* sm_count, int32_t* cc_major, 
   if (sm_count) *sm_count = ctx->sm_count;
   if (cc_major) *cc_major = ctx->cc_major;
   if (cc_minor) *cc_minor = ctx->cc_minor;
+  return PDB_OK;
+}
+
+int pdb_set_reproducible(pdb_context* c, int on) {
+  if (!c) return PDB_ERR_INVALID;
+  Context* ctx = reinterpret_cast<Context*>(c);
+  if (on != 0 && on != 1) return ctx->fail(PDB_ERR_INVALID, "pdb_set_reproducible: on = %d, expected 0 or 1", on);
+  ctx->reproducible = on == 1;  // read when work is enqueued
   return PDB_OK;
 }
 
@@ -460,6 +471,12 @@ __global__ void __launch_bounds__(kGgsThreads, 1)
 ggs_entry(const __grid_constant__ GgsBatch batch, const __grid_constant__ GgsParams P) {
   ggs_body<kEval, kPaired, kProbe, kLean>(batch.prob[blockIdx.x / P.ctas_per_problem], P);
 }
+// the reproducible instantiation (pdb_set_reproducible): a kernel of its own, so that the default ones keep their names and code
+template <bool kPaired>
+__global__ void __launch_bounds__(kGgsThreads, 1)
+ggs_entry_repro(const __grid_constant__ GgsBatch batch, const __grid_constant__ GgsParams P) {
+  ggs_body<false, kPaired, false, false, true>(batch.prob[blockIdx.x / P.ctas_per_problem], P);
+}
 
 // segs_fit: every CTA of every sequence in the batch touches at most kGgsMaxSeg segments (ggs_lean_fits)
 template <bool kEval, bool kPaired, bool kProbe = false>
@@ -469,8 +486,9 @@ int launch_ggs_chunk(Context* ctx, const GgsBatch& batch, int nprob, int max_fra
     if (batch.prob[0].dbg_clock) return launch_ggs_chunk<kEval, kPaired, true>(ctx, batch, nprob, max_frames, max_rounds, P, segs_fit, st);
   }
   const int cpp = P.ctas_per_problem;  // ggs_plan
+  const bool repro = !kEval && ctx->reproducible;  // enqueue_ggs has chosen the slot exchange and no probe
   // shared-memory match cache: everything beyond the fixed per-frame state, in rounds of 512 B
-  const size_t fixed = ggs_smem_fixed_bytes(max_frames);
+  const size_t fixed = ggs_smem_fixed_bytes(max_frames, repro);
   const size_t budget = ctx->smem_optin > fixed + 1024 ? ctx->smem_optin - fixed - 1024 : 0;
   const long long rounds_per_cta = ggs_rounds_per_cta(max_rounds, cpp, kPaired);
   // PDB_GGS_FORCE_STREAM=1 disables the shared-memory-resident mode (tests exercise the streaming ring with it)
@@ -480,10 +498,12 @@ int launch_ggs_chunk(Context* ctx, const GgsBatch& batch, int nprob, int max_fra
   P.ring = resident ? 0 : 1;
   // the lean instantiation serves the case it was specialised for; PDB_GGS_LEAN=0 keeps the general kernel (tests compare the two)
   const char* lean_env = getenv("PDB_GGS_LEAN");
-  const bool lean = !kEval && resident && segs_fit && P.xch_mode == 1 && !(lean_env && lean_env[0] == '0');
-  const void* kernel = lean ? (const void*)ggs_entry<kEval, kPaired, kProbe, !kEval> : (const void*)ggs_entry<kEval, kPaired, kProbe, false>;
+  const bool lean = !kEval && !repro && resident && segs_fit && P.xch_mode == 1 && !(lean_env && lean_env[0] == '0');
+  const void* kernel = repro ? (const void*)ggs_entry_repro<kPaired>
+                       : lean ? (const void*)ggs_entry<kEval, kPaired, kProbe, !kEval> : (const void*)ggs_entry<kEval, kPaired, kProbe, false>;
   const size_t smem = fixed + (resident ? (size_t)rounds_per_cta * 512 : (size_t)kRingBytes);
-  size_t& attr_bytes = ctx->attr->ggs[(kEval ? 1 : 0) + (kPaired ? 2 : 0) + (kProbe ? 4 : 0) + (lean ? 8 : 0)];
+  size_t& attr_bytes = repro ? ctx->attr->ggs_repro[kPaired ? 1 : 0]
+                             : ctx->attr->ggs[(kEval ? 1 : 0) + (kPaired ? 2 : 0) + (kProbe ? 4 : 0) + (lean ? 8 : 0)];
   if (smem > attr_bytes) {
     PDB_CUDA(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_bytes = smem;
@@ -585,7 +605,7 @@ int enqueue_ggs(Context* ctx, pdb_matches* const* problems, int batch, int frame
       max_rounds = max_rounds > m->rounds ? max_rounds : m->rounds;
     }
     ggs_plan(ctx, nb, max_rounds, &P.ctas_per_problem, &P.xch_group);
-    P.xch_mode = ggs_xch_mode();
+    P.xch_mode = ctx->reproducible ? 0 : ggs_xch_mode();  // the one-hop exchange adds in arrival order
     bool segs_fit = true;
     for (int i = 0; i < nb; ++i) {
       const Matches* m = reinterpret_cast<const Matches*>(problems[b0 + i]);
@@ -604,7 +624,7 @@ int enqueue_ggs(Context* ctx, pdb_matches* const* problems, int batch, int frame
       p.xch2 = p.xch1 + 2 * (size_t)P.ctas_per_problem * ggs_xch_words(m->frames);
       p.acc = reinterpret_cast<float*>(ws + ggs_ws_slots_bytes(max_frames, P.ctas_per_problem, P.xch_group));
       p.stats = stats_dev ? stats_dev + (b0 + i) : nullptr;
-      p.dbg_clock = (ctx->ggs_clock && !ctx->den_clock && batch == 1) ? ctx->ggs_clock : nullptr;
+      p.dbg_clock = (ctx->ggs_clock && !ctx->den_clock && batch == 1 && !ctx->reproducible) ? ctx->ggs_clock : nullptr;
       ws += ggs_ws_per_problem(max_frames, P.ctas_per_problem, P.xch_group);
     }
     const int layout = reinterpret_cast<const Matches*>(problems[b0])->layout;

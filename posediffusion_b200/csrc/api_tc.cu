@@ -152,8 +152,9 @@ int enqueue_tc_linear(Context* ctx, const float* X, const float* W, TcEpilogue E
     // LayerNorm statistics come out of the X tiles inside the kernel (E.stats, requested by the caller).
     const int tiles = (E.O / 64) * ((E.S + kTcBM - 1) / kTcBM), num_kb = E.K / kTcBK;
     E.splits = 1;
+    // (reproducible mode: no split, every output element is one CTA's dot product in k order)
     const bool in_place = E.residual == E.Y && E.ldr == E.ldy && !E.relu && !E.gelu && !E.colsum;
-    if (in_place)
+    if (in_place && !ctx->reproducible)
       for (int s : {8, 4, 2})
         if (num_kb % s == 0 && num_kb / s >= 2 && tiles * s <= ctx->sm_count) {
           E.splits = s;
@@ -352,7 +353,8 @@ int enqueue_denoiser_tc(Context* ctx, const DenoiserDev& dev, DenoiserRun run, c
   std::vector<size_t> key = {(size_t)S, (size_t)B, (size_t)N, (size_t)run.guide_below, (size_t)ctx->den_ws, (size_t)run.x,
                              (size_t)run.draws, (size_t)run.trail, (size_t)run.eps_out, (size_t)run.x0_out, (size_t)run.mean_out,
                              (size_t)w->tc_arena, (size_t)dev.tproj, (size_t)dev.sched, (size_t)ctx->tc_swap, (size_t)stats_qkv, (size_t)stats_ff1,
-                             (size_t)tc_linear_small(ctx, S, kDM), (size_t)(ctx->tc_pdl && S <= 320)};  // launcher regime: the captured kernels differ
+                             (size_t)tc_linear_small(ctx, S, kDM), (size_t)(ctx->tc_pdl && S <= 320),  // launcher regime: the captured kernels differ
+                             (size_t)ctx->reproducible};  // split-K or not
   if (!ctx->tc_graph || ctx->tc_graph_key != key) {
     if (ctx->tc_graph) { cudaGraphExecDestroy(ctx->tc_graph); ctx->tc_graph = nullptr; }
     if (!ctx->tc_capture_stream) PDB_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->tc_capture_stream, cudaStreamNonBlocking));

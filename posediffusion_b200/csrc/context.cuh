@@ -19,6 +19,7 @@ struct VitWeights;       // api_vit.cu
 // launches with).
 struct KernelAttrs {
   size_t ggs[16] = {}, den[16] = {}, att = 0;
+  size_t ggs_repro[2] = {0, 0};  // the reproducible GGS instantiation, plain / paired layout
   bool tc = false, tc128 = false, tc_deep = false;
   bool tc_swap[3] = {false, false, false};  // swap-AB instantiations (32 / 64 / 96 tokens on the N side)
   size_t vit_att[2] = {0, 0};  // the forward attention kernel's copy in api_vit.cu / api_vit_train.cu
@@ -75,6 +76,9 @@ struct Context {
   size_t vit_ws_bytes = 0;
   int ggs_layout = 1;       // stream layout of match sets packed on this context (ggs_layout.cuh): 0 plain, 1 paired (default)
   int denoiser_engine = 0;  // 0 auto, 1 fp32 persistent kernel, 2 wgmma/TMA tiles (TF32)
+  // pdb_set_reproducible: the same bits on every call (GGS with fixed-order sums and the slot exchange, tensor-core GEMMs without
+  // split-K); read when work is enqueued
+  bool reproducible = false;
   // optional per-kernel timing (bench.py roofline): event pairs per launch, kind 0 = GGS, 1 = denoiser
   bool profiling = false;
   struct Timed { cudaEvent_t a, b; int kind; };

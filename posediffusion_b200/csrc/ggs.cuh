@@ -77,13 +77,16 @@ __host__ __device__ inline int ggs_xch_words(int frames) { return frames * 7 + k
 __host__ __device__ inline int ggs_xch_groups(int cpp, int group) { return group >= cpp ? 0 : (cpp + group - 1) / group; }
 
 constexpr int kGgsFixedFloatsPerFrame = 2 * 9 + 4 * 9 + 4 + 18 + 14;  // pose, vel, R, A, Rt, At, fl, inr, gAt|gRt, partial + summed gradient
+// Reproducible instantiation only: one stage-1 partial per (warp, segment) -- slot segment + warp, kGgsMaxSeg + kGgsWarps - 1
+// slots -- and each warp's segment range {first, last} (ggs_body, kRepro).
+constexpr int kGgsReproBytes = ((kGgsMaxSeg + kGgsWarps - 1) * kSegAcc * 4 + kGgsWarps * 8 + 127) / 128 * 128;
 
-__host__ __device__ inline size_t ggs_smem_fixed_bytes(int frames) {
+__host__ __device__ inline size_t ggs_smem_fixed_bytes(int frames, bool repro = false) {
   size_t bytes = sizeof(float) * ((size_t)frames * kGgsFixedFloatsPerFrame + 128 + (size_t)kGgsMaxSeg * kSegAcc);
   bytes += kGgsMaxSeg * sizeof(int);         // segment valid counts
   bytes += 2 * (size_t)frames * sizeof(int);  // exchange plan: contributors per frame, own frames
   bytes += (kGgsMaxSeg + 1) * sizeof(int4);  // segment descriptors
-  return (bytes + 127) / 128 * 128;
+  return (bytes + 127) / 128 * 128 + (repro ? kGgsReproBytes : 0);
 }
 
 // Element-wise float2 arithmetic, one match per component.  Correctly rounded FMA / multiply / add: __fmul_rn and __fadd_rn are
@@ -271,9 +274,15 @@ inline bool ggs_lean_fits(const int4* segs, int nseg, long long rounds, int cpp,
 // kLean: the instantiation of the common case (config 3): resident slice, at most kGgsMaxSeg segments per CTA, one-hop
 // exchange, optimisation.  The host picks it only when all of that holds (ggs_lean_fits); the ring, register-stream and
 // multi-chunk stage-1 paths and the slot exchange are compiled out, which keeps the kernel free of spills and its loop small.
-template <bool kEval, bool kPaired = false, bool kProbe = false, bool kLean = false>
+// kRepro: the reproducible instantiation (pdb_set_reproducible).  Every float sum has a fixed order, so the pose and the
+// statistics do not depend on how warps and CTAs are scheduled: stage 1 stores one partial per (warp, segment) instead of adding
+// into the segment's accumulator, and a pass sums each segment's partials in warp order; stage 2a runs frame-major, every frame
+// adding its segments' adjoints in segment order; the stage-2b scalars of more than one frame warp go through per-warp slots; the
+// exchange is the flag-carrying slot exchange (fixed order; the host sets xch_mode 0).  Integer sums stay atomic.
+template <bool kEval, bool kPaired = false, bool kProbe = false, bool kLean = false, bool kRepro = false>
 __device__ __forceinline__ void ggs_body(const GgsProblem& pr, const GgsParams& P) {
   static_assert(!(kLean && kEval), "the lean instantiation is optimisation only");
+  static_assert(!(kRepro && (kEval || kProbe || kLean)), "the reproducible instantiation is optimisation only, without probe");
 #ifdef PDB_EMU  // tests/host/cuda_emu.h (CPU emulation of this kernel, test harness only): dynamic shared memory of this CTA
   unsigned char* const smem_raw = emu::g_cta->smem;
 #else
@@ -303,7 +312,9 @@ __device__ __forceinline__ void ggs_body(const GgsProblem& pr, const GgsParams& 
   int* s_scnt = reinterpret_cast<int*>(s_sacc + kGgsMaxSeg * kSegAcc);
   int* s_expect = s_scnt + kGgsMaxSeg;  // [N] CTAs of this sequence that contribute to frame n (one-hop exchange)
   int* s_mine = s_expect + N;           // [N] 1 if this CTA's segments touch frame n
-  float4* s_pts = reinterpret_cast<float4*>(smem_raw + ggs_smem_fixed_bytes(N));
+  float* s_wacc = reinterpret_cast<float*>(smem_raw + ggs_smem_fixed_bytes(N));  // kRepro: [kGgsMaxSeg + kGgsWarps - 1][kSegAcc]
+  int2* s_wrng = reinterpret_cast<int2*>(s_wacc + (kGgsMaxSeg + kGgsWarps - 1) * kSegAcc);  // kRepro: [kGgsWarps] chunk-relative
+  float4* s_pts = reinterpret_cast<float4*>(smem_raw + ggs_smem_fixed_bytes(N, kRepro));
   __shared__ int s_cta_cnt;
 
   // ---- static work partition: rounds -> CTAs -> warps ----
@@ -458,6 +469,7 @@ __device__ __forceinline__ void ggs_body(const GgsProblem& pr, const GgsParams& 
           if (tid <= nchunk) s_seg[tid] = __ldg(&pr.segs[cs + tid]);
           __syncthreads();
         }
+        int w_first = kGgsMaxSeg, w_last = -1;  // kRepro: the chunk-relative segments this warp visits
         // ---- stage 1: stream the matches of this warp's rounds ----
         {
           if (use_ring) {
@@ -505,7 +517,13 @@ __device__ __forceinline__ void ggs_body(const GgsProblem& pr, const GgsParams& 
                 nval = __reduce_add_sync(0xffffffffu, (int)g[11]);  // per-lane counts are exact small integers
                 const float tot = warp_reduce16(g, lane);
                 const int slot = warp_reduce16_slot(lane);
-                if (!(lane & 1) && slot < 11) atomicAdd(&s_sacc[(s - cs) * kSegAcc + slot], tot);
+                if constexpr (kRepro) {
+                  if (!(lane & 1) && slot < 11) s_wacc[(s - cs + warp) * kSegAcc + slot] = tot;
+                  w_first = min(w_first, s - cs);
+                  w_last = s - cs;
+                } else if (!(lane & 1) && slot < 11) {
+                  atomicAdd(&s_sacc[(s - cs) * kSegAcc + slot], tot);
+                }
                 if (lane == 0 && nval) atomicAdd(&s_scnt[s - cs], nval);
               };
               begin_segment();
@@ -698,16 +716,79 @@ __device__ __forceinline__ void ggs_body(const GgsProblem& pr, const GgsParams& 
             nval = __reduce_add_sync(0xffffffffu, (int)g[11]);  // per-lane counts are exact small integers
             const float tot = warp_reduce16(g, lane);
             const int slot = warp_reduce16_slot(lane);
-            if (!(lane & 1) && slot < 11) atomicAdd(&s_sacc[(s - cs) * kSegAcc + slot], tot);
+            if constexpr (kRepro) {
+              if (!(lane & 1) && slot < 11) s_wacc[(s - cs + warp) * kSegAcc + slot] = tot;
+              w_first = min(w_first, s - cs);
+              w_last = s - cs;
+            } else if (!(lane & 1) && slot < 11) {
+              atomicAdd(&s_sacc[(s - cs) * kSegAcc + slot], tot);
+            }
             if (lane == 0 && nval) atomicAdd(&s_scnt[s - cs], nval);
             r = r_end;
             ++s;
           }
           }
         }
+        if constexpr (kRepro) {
+          if (lane == 0) s_wrng[warp] = make_int2(w_first, w_last);
+        }
         __syncthreads();
+        if constexpr (kRepro) {
+          // Fixed-order pass over stage 1: segment sl = the sum of its partials in warp order.  A warp's rounds are contiguous and
+          // follow those of the previous warp, so two warps share at most one segment and slot sl + w belongs to (w, sl) alone.
+          for (int sl = warp; sl < nchunk; sl += kGgsWarps) {
+            if (lane < 11) {
+              float v = 0.f;
+              for (int w = 0; w < kGgsWarps; ++w) {
+                const int2 wr = s_wrng[w];
+                if (wr.x <= sl && sl <= wr.y) v += s_wacc[(sl + w) * kSegAcc + lane];
+              }
+              s_sacc[sl * kSegAcc + lane] = v;
+            }
+          }
+          __syncthreads();
+        }
         if (kProbe && pr.dbg_clock && tid == 0) ck1a = clock64();
         // ---- stage 2a: per-pair adjoint, one warp per segment, 18 lanes x 2 outputs; leaves the slots zeroed ----
+        if constexpr (kRepro) {
+          // frame-major: one warp per frame walks the chunk's segments in order; lanes 0..8 add the adjoints of the segments in
+          // which the frame is side 0, lanes 9..17 those in which it is side 1, then lane e adds lane e + 9's sums to its own
+          const int side = lane >= 9, e = (lane - side * 9) % 9, i = e / 3, j = e - i * 3;
+          for (int n = warp; n < N; n += kGgsWarps) {
+            float oA = 0.f, oR = 0.f;
+            if (lane < 18) {
+              for (int sl = 0; sl < nchunk; ++sl) {
+                const int4 sd = s_seg[sl];
+                if ((side ? sd.w : sd.z) != n) continue;
+                const float* G = s_sacc + sl * kSegAcc;
+                float g3[3], a, r;
+#pragma unroll
+                for (int k = 0; k < 3; ++k) g3[k] = side ? G[k * 3 + i] : G[i * 3 + k];
+                const int other = side ? sd.z : sd.w;
+                pair_adjoint_entry(g3, s_At + other * 9, s_Rt + other * 9, j, &a, &r);
+                oA += a;
+                oR += r;
+              }
+            }
+            oA += __shfl_sync(0xffffffffu, oA, lane + 9);
+            oR += __shfl_sync(0xffffffffu, oR, lane + 9);
+            if (lane < 9) {
+              s_fg[n * 18 + e] += oA;
+              s_fg[n * 18 + 9 + e] += oR;
+            }
+          }
+          if (tid == kGgsThreads - 1) {  // the scalars in segment order; the counts are integers
+            float clamp_sum = 0.f;
+            int cnt = 0;
+            for (int sl = 0; sl < nchunk; ++sl) {
+              clamp_sum += s_sacc[sl * kSegAcc + 9];
+              cnt += s_scnt[sl];
+              s_scnt[sl] = 0;
+            }
+            s_misc[4] += clamp_sum;
+            s_cta_cnt += cnt;
+          }
+        } else {
         for (int sl = warp; sl < nchunk; sl += kGgsWarps) {
           const int4 sd = s_seg[sl];
           float* G = s_sacc + sl * kSegAcc;
@@ -736,6 +817,7 @@ __device__ __forceinline__ void ggs_body(const GgsProblem& pr, const GgsParams& 
           } else if (lane == 19 && kEval) {
             atomicAdd(&s_misc[5], gs);
           }
+        }
         }
         if (kLean) break;  // one chunk
       }
@@ -766,6 +848,9 @@ __device__ __forceinline__ void ggs_body(const GgsProblem& pr, const GgsParams& 
           if (N <= 32) {
 #pragma unroll
             for (int k = 0; k < 4; ++k) s_misc[8 + k] = k4[k];
+          } else if constexpr (kRepro) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) s_misc[48 + warp * 4 + k] = k4[k];  // per-warp slots, summed in warp order below
           } else {
 #pragma unroll
             for (int k = 0; k < 4; ++k) atomicAdd(&s_misc[8 + k], k4[k]);
@@ -773,13 +858,24 @@ __device__ __forceinline__ void ggs_body(const GgsProblem& pr, const GgsParams& 
         }
       }
       __syncthreads();
+      if constexpr (kRepro) {
+        static_assert(kMaxFrames <= 4 * 32, "four frame warps: s_misc[48..63]");
+        if (N > 32) {
+          if (tid < 4) {
+            float v = 0.f;
+            for (int w = 0; w * 32 < N; ++w) v += s_misc[48 + w * 4 + tid];
+            s_misc[8 + tid] = v;
+          }
+          __syncthreads();
+        }
+      }
       if (kProbe && pr.dbg_clock && tid == 0) ck2 = clock64();
       // ================= exchange: all-reduce of the partial gradient over the CTAs of this sequence =================
       if constexpr (kLean) {
         const float g_fx = (-s_misc[8] + cx * s_misc[10]) / (fpx * fpx), g_fy = (-s_misc[9] + cy * s_misc[11]) / (fpy * fpy);
         ggs_exchange_acc<kEval>(pr.acc, cpp, cta, N, it_global, s_part, s_misc, s_cta_cnt, g_fx, g_fy, s_gsum, s_expect, s_mine);
       } else {
-        ggs_exchange<kEval>(pr.xch1, pr.xch2, P.xch_mode == 1 ? pr.acc : nullptr, cpp, cta, P.xch_group, N, it_global, s_part, s_misc, s_cta_cnt,
+        ggs_exchange<kEval>(pr.xch1, pr.xch2, !kRepro && P.xch_mode == 1 ? pr.acc : nullptr, cpp, cta, P.xch_group, N, it_global, s_part, s_misc, s_cta_cnt,
                             (-s_misc[8] + cx * s_misc[10]) / (fpx * fpx), (-s_misc[9] + cy * s_misc[11]) / (fpy * fpy), s_gsum, s_expect, s_mine);
       }
       ++it_global;
